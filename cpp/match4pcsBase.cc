@@ -427,7 +427,7 @@ void Match4PCSBase::RunSpeculation() {
       lanes_stale_ = true;
     }
     if (lanes_stale_) {
-      for (s4g_ctx* lane : lanes_) UploadCloudsTo(lane);  // (sequential: the form that has run on the B200)
+      for (s4g_ctx* lane : lanes_) UploadCloudsTo(lane);  // (sequential: the form the GPU tests run)
       lanes_stale_ = false;
     }
   }

@@ -1,5 +1,5 @@
 /*
- * s4g.h -- C ABI of libs4g.so, the B200-native (sm_100a) implementation of the Super4PCS
+ * s4g.h -- C ABI of libs4g.so, the H100-native (sm_90a) implementation of the Super4PCS
  * congruent-set extraction + LCP verification hot path.
  *
  * The reference (nmellado/Super4PCS) has no FFI: its drop-in boundary is the C++ class

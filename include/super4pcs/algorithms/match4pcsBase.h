@@ -6,7 +6,7 @@
 // same protected state names (h:120-165) so that Testing::TestMatcher-style subclasses (reference
 // tests/testing.h:71-154) compile unchanged.  What is different is underneath: the kd-tree of
 // sampled P (reference accelerators/kdtree.h) is replaced by the device grid behind the C ABI of
-// include/s4g.h, and every hot stage (pairs, quads, rigid fit, Verify) runs as sm_100a CUDA.
+// include/s4g.h, and every hot stage (pairs, quads, rigid fit, Verify) runs as sm_90a CUDA.
 // The host side below keeps the reference's control flow, RNG consumption order (SURVEY.md A.6)
 // and float/double mixing (A.1-A.7) so that results are identical on the same inputs.
 #ifndef SUPER4PCS_B200_ALGO_MATCH4PCSBASE_H_
@@ -213,7 +213,7 @@ class Match4PCSBase {
   void LogTimings() const;
 
   // ---- speculative multi-base execution (SURVEY.md section 8, row f1)
-  // The reference tries one base at a time (hpp:236-256); a small sample keeps a B200 idle that
+  // The reference tries one base at a time (hpp:236-256); a small sample keeps a GPU idle that
   // way (a base is a handful of tiny kernels and size read-backs).  Base selection depends only on
   // the RNG and on sampled P, and a base's best candidate does not depend on best_LCP_ (hpp:363-497
   // verifies every gate-passing quad), so the next few bases are selected ahead -- in RNG order --

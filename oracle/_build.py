@@ -1,12 +1,40 @@
-"""TEST INFRASTRUCTURE ONLY: builds oracle/liboracle_port.so and, when /root/reference is
-present, oracle/_ref/liboracle_ref.so (see oracle/Makefile)."""
+"""TEST INFRASTRUCTURE ONLY: builds oracle/liboracle_port.so and, when the reference is present,
+oracle/_ref/liboracle_ref.so (see oracle/Makefile) and the staged copy oracle/_ref/reference (stage_reference)."""
 import os
+import shutil
 import subprocess
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 PORT_SO = os.path.join(HERE, "liboracle_port.so")
 REF_SO = os.path.join(HERE, "_ref", "liboracle_ref.so")
-REFERENCE_ROOT = os.environ.get("S4_REFERENCE_ROOT", "/root/reference")
+# the parts of the reference that the C++ layer and the GPU-side test binaries compile against, staged by
+# stage_reference() so that they travel with oracle/_ref to a machine without the reference tree
+STAGED_REF = os.path.join(HERE, "_ref", "reference")
+STAGED_PARTS = (("3rdparty", "Eigen"), ("demos",), ("tests", "externalAppTest"))
+_SOURCE_ROOT = os.environ.get("S4_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = _SOURCE_ROOT if os.path.isdir(_SOURCE_ROOT) or not os.path.isdir(STAGED_REF) else STAGED_REF
+
+
+def stage_reference():
+    """Copies STAGED_PARTS of the reference (Eigen, the host-side dependency of the C++ API; the demo mains, the PCL
+    wrapper and the MeshLab plugin; the packaging test's main) into oracle/_ref/reference when the reference is present
+    and they are not staged yet.  Returns the root the C++ layer and the test binaries are to be built against: the
+    reference itself, else the staged copy, else None."""
+    if os.path.isdir(os.path.join(_SOURCE_ROOT, "3rdparty", "Eigen", "Eigen")) and \
+            os.path.realpath(_SOURCE_ROOT) != os.path.realpath(STAGED_REF):
+        for part in STAGED_PARTS:
+            dst = os.path.join(STAGED_REF, *part)
+            if not os.path.isdir(dst):
+                tmp = dst + ".tmp"
+                shutil.rmtree(tmp, ignore_errors=True)
+                shutil.copytree(os.path.join(_SOURCE_ROOT, *part), tmp, copy_function=shutil.copyfile)
+                for dp, dns, _ in os.walk(tmp):
+                    os.chmod(dp, 0o755)
+                os.rename(tmp, dst)
+        return _SOURCE_ROOT
+    if os.path.isdir(os.path.join(STAGED_REF, "3rdparty", "Eigen", "Eigen")):
+        return STAGED_REF
+    return None
 
 
 def _stale(target, sources):

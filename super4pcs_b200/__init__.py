@@ -1,4 +1,4 @@
-"""super4pcs_b200 -- B200-native (sm_100a) Super4PCS congruent-set extraction + LCP verification.
+"""super4pcs_b200 -- H100-native (sm_90a) Super4PCS congruent-set extraction + LCP verification.
 
 The product is `lib/libs4g.so` (hand-written CUDA behind the C ABI of include/s4g.h) and the
 header-compatible C++ layer in include/super4pcs/.  This Python package is the thin ctypes

@@ -1,4 +1,4 @@
-"""Builds super4pcs_b200/lib/libs4g.so (hand-written sm_100a CUDA + the extern "C" ABI of
+"""Builds super4pcs_b200/lib/libs4g.so (hand-written sm_90a CUDA + the extern "C" ABI of
 include/s4g.h) IN-TREE with nvcc.  Cross-compiles without a GPU."""
 import concurrent.futures as cf
 import os
@@ -15,7 +15,7 @@ SOURCES = ["context.cu", "verify.cu", "rigid.cu", "pairs.cu", "quads.cu", "sampl
 
 NVCC_FLAGS = [
     "-std=c++17", "-O3",
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "-fmad=false",            # parity: the reference binary has no FMA contraction (SURVEY B.1/B.3)
     "-Xcompiler", "-fPIC",
@@ -78,7 +78,7 @@ def build_lib(force=False, verbose=False, extra_flags=()):
         outs = list(ex.map(run, jobs))
     objs = [os.path.join(OBJ, s.replace(".cu", ".o")) for s in srcs]
     if jobs or force or _stale(LIB, objs):
-        run([nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a",
+        run([nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a",
              "-Xcompiler", "-fPIC", "-cudart", "static"])
     with open(stamp, "w") as f:
         f.write(defines)

@@ -10,8 +10,8 @@
 the test side, not here.)
 
 Eigen (a host-side dependency of the public API types, e.g. Eigen::Ref<Matrix4f>) is taken from
-S4_EIGEN_ROOT or the reference's vendored copy; without it (the GPU box) the prebuilt binaries that
-travelled with the repo are used as they are.
+S4_EIGEN_ROOT or the vendored copy of the reference named by S4_REFERENCE_ROOT (the driver's build() points it at a
+staged copy where the reference tree is absent); without any, binaries built earlier are used as they are.
 """
 import os
 import subprocess

@@ -515,8 +515,8 @@ extern "C" int s4g_set_cloud_p(s4g_ctx* ctx, const float* xyz, int n, float delt
   g.csat = nullptr;
   g.vocc = nullptr;
   // coarse blocks for the tile cull: as fine as a 1M-entry (4 MB) summed-area table allows -- 4x4x4 cells at 1M points.
-  // (A/B on the B200, S4G_CSHIFT_MIN: 2x2x2-cell blocks cull 86.0 % of the (warp, candidate) pairs instead of 83.4 %, but
-  // their 29 MB table costs more in L2 misses than the extra pairs cost in instructions: 5.52 vs 5.40 ms per launch.)
+  // (2x2x2-cell blocks cull a few more (warp, candidate) pairs, but their table is 8x larger and competes with the rest
+  // of the working set for L2; S4G_CSHIFT_MIN selects coarser blocks for an A/B.)
   int cshift_min = 1;
   if (const char* e = std::getenv("S4G_CSHIFT_MIN")) cshift_min = std::max(1, std::min(11, std::atoi(e)));   // A/B knob: coarser cull blocks
   for (g.cshift = cshift_min; g.cshift < 12; ++g.cshift) {

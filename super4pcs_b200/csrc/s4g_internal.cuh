@@ -72,7 +72,7 @@ struct s4g_ctx {
   cudaStream_t stream = nullptr;
   cudaStream_t own_stream = nullptr;
   std::string err;
-  int sm_count = 148;
+  int sm_count = 132;
 
   // ---- P side
   int nP = 0;

@@ -9,10 +9,10 @@
 //   d^2  = dx^2 + (dy^2 + dz^2)                                     (kdtree.h:417)
 //   hit  = d^2 <= delta*delta                                       (kdtree.h:418, cc:522)
 //
-// Schedule (B200).  The working set (Q 16 MB, delta-field 27 + 35 MB, sorted P 16 MB, cellStart, brick
-// tables, a 4 MB summed-area table: ~110 MB at 1M points) is mostly L2-resident; the kernel is bound by
-// instruction issue and L2 latency, so the design minimises instructions per (query, candidate) pair -- by
-// deciding as many pairs as possible from pre-computed bits instead of point tests:
+// Schedule.  The working set (Q 16 MB, delta-field 27 + 35 MB, sorted P 16 MB, cellStart, brick
+// tables, a 4 MB summed-area table: ~110 MB at 1M points) is about twice the 50 MB L2 of an H100, but the
+// Morton order of the queries keeps the look-ups of a warp local; the design minimises instructions and look-ups
+// per (query, candidate) pair -- by deciding as many pairs as possible from pre-computed bits instead of point tests:
 //  * sampled_Q is streamed in Morton order, one coalesced float4 per thread per tile; a CTA stages a
 //    chunk of 16 candidate transforms and owns 8 tiles of 128 queries.
 //  * phase 0 (two levels, one thread per (tile, candidate), then one per (surviving pair, warp)): the bounding sphere of

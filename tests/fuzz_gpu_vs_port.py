@@ -1,5 +1,4 @@
-"""TEST INFRASTRUCTURE, not collected by pytest; needs a B200 (written at the end of round 1 for the first GPU session of
-round 2): time-boxed fuzz of every device stage through the C ABI against the oracle port -- pairs with random filters,
+"""TEST INFRASTRUCTURE, not collected by pytest; needs an H100: time-boxed fuzz of every device stage through the C ABI against the oracle port -- pairs with random filters,
 quads, rigid fits, Verify counts, TryCongruentSet winners -- over random clouds / deltas / bases, including tiny and
 degenerate clouds.  The CPU-side twin (port vs compiled reference) is tests/fuzz_port_vs_reference.py.
   python tests/fuzz_gpu_vs_port.py [seed] [seconds]"""

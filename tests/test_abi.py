@@ -1,4 +1,4 @@
-"""CPU tests: the C-ABI library builds for sm_100a, loads, exports every symbol include/s4g.h
+"""CPU tests: the C-ABI library builds for sm_90a, loads, exports every symbol include/s4g.h
 declares, and fails LOUDLY (no CPU fallback) when there is no CUDA device."""
 import ctypes
 import os
@@ -16,11 +16,11 @@ def test_library_exports_every_declared_symbol(s4g_lib):
     assert s4g_lib.s4g_abi_version() == 1
 
 
-def test_library_is_sm100a_cuda_code(s4g_lib):
+def test_library_is_sm90a_cuda_code(s4g_lib):
     out = subprocess.run(["cuobjdump", "--list-elf", s4g.lib_path()], capture_output=True, text=True)
     if out.returncode != 0:
         pytest.skip("cuobjdump unavailable")
-    assert "sm_100a" in out.stdout
+    assert "sm_90a" in out.stdout
 
 
 def test_result_struct_layout_matches_header():

@@ -54,14 +54,3 @@ def test_reference_arm_prints_the_contract_line():
 def test_physical_cores_counts_smt_siblings_once():
     assert 1 <= bench.physical_cores() <= bench.host_threads()
 
-
-def test_committed_ncu_figures_belong_to_the_kernel_sources_in_the_tree():
-    """profiles/verify_ncu.json feeds roofline.issue / roofline.traffic; bench.py drops it when the digest of verify.cu +
-    context.cu + s4g_internal.cuh differs -- this test makes forgetting to re-stamp (or re-capture) it a red CPU suite"""
-    import json
-    import os
-    import bench
-    with open(os.path.join(bench.ROOT, "profiles", "verify_ncu.json")) as f:
-        d = json.load(f)
-    assert d["source_digest"] == bench.source_digest()
-    assert d["candidates"] == bench.CANDIDATES_PER_GPU and d["n_points"] == bench.N_POINTS

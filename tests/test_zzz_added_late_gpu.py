@@ -1,5 +1,4 @@
-"""GPU tests written after the round-1 GPU budget was spent: they run for the first time in the driver's round-end pass and
-are therefore collected AFTER every test that has already been green on a B200 (file name order).  The a1 normalisation,
+"""GPU tests collected AFTER every other GPU test (file name order).  The a1 normalisation,
 the GPU variant of the randomised pipeline sweep and the exact-order tie cases (see tests/test_host_logic_cpu.py for the
 CPU twins on the oracle stand-in)."""
 import os
