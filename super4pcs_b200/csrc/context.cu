@@ -93,7 +93,10 @@ extern "C" int s4g_create(int device, s4g_ctx** out_ctx) {
         return S4G_ERR_CUDA;
       }
   cudaDeviceProp prop;
-  if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) ctx->sm_count = prop.multiProcessorCount;
+  if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) {
+    ctx->sm_count = prop.multiProcessorCount;
+    if (prop.l2CacheSize > 0) ctx->l2_bytes = prop.l2CacheSize;
+  }
   {
     // keep freed scratch in the pool instead of returning it to the driver at every synchronisation
     cudaMemPool_t pool = nullptr;
@@ -121,10 +124,10 @@ extern "C" void s4g_destroy(s4g_ctx* ctx) {
   DevBuf* all[] = {&ctx->dP, &ctx->dPsorted, &ctx->dTop, &ctx->dCellStart, &ctx->dCsat, &ctx->dVtop, &ctx->dVox, &ctx->dVocc, &ctx->dVbase, &ctx->dVfine, &ctx->dQtiles, &ctx->dQmside, &ctx->dQ, &ctx->dQmorton,
                    &ctx->dQn, &ctx->dQrgb, &ctx->dQunit, &ctx->dQgroups, &ctx->dPairs[0], &ctx->dPairs[1], &ctx->dQuads,
                    &ctx->dScratchA, &ctx->dScratchB, &ctx->dScratchC, &ctx->dScratchD, &ctx->dCub,
-                   &ctx->dT12, &ctx->dRms, &ctx->dOk, &ctx->dCandIdx, &ctx->dCounts, &ctx->dResult,
+                   &ctx->dRms, &ctx->dOk, &ctx->dCandIdx, &ctx->dCounts, &ctx->dResult,
                    &ctx->dMisc, &ctx->bArgs, &ctx->bCounts, &ctx->bPairKeys[0], &ctx->bPairKeys[1], &ctx->bQKeys[0], &ctx->bQKeys[1],
                    &ctx->bQVals[0], &ctx->bQVals[1], &ctx->bQCnt, &ctx->bQuadKeys[0], &ctx->bQuadKeys[1], &ctx->bQuads, &ctx->bMisc,
-                   &ctx->bResults};
+                   &ctx->bResults, &ctx->dQpatch, &ctx->dVrec, &ctx->dVsort};
   for (DevBuf* b : all) free_buf(ctx, *b);
   cudaStreamSynchronize(ctx->stream);
   if (ctx->hPinned) cudaFreeHost(ctx->hPinned);
@@ -660,16 +663,20 @@ extern "C" int s4g_get_grid_stats(s4g_ctx* ctx, double* out6) {
   unsigned long long ne = 0;
   S4G_CUDA(cudaMemcpyAsync(&ne, ctx->dMisc.p, 8, cudaMemcpyDeviceToHost, ctx->stream));
   S4G_CUDA(cudaStreamSynchronize(ctx->stream));
-  long long ntop = (long long)ctx->grid.tbx * ctx->grid.tby * ctx->grid.tbz;
   out6[0] = ctx->cell_h;
   out6[1] = (double)ctx->nBricks;
   out6[2] = (double)(1 << ctx->grid.bshift);
   out6[3] = (double)ctx->nCells;
   out6[4] = ne ? (double)ctx->nP / (double)ne : 0.0;
-  out6[5] = (double)ctx->nP * 16.0 + (double)(ctx->nCells + 1) * 4.0 + (double)ntop * 4.0 +
-            (double)ntop * 4.0 + (double)(ctx->nVBricks << (3 * ctx->grid.bshift)) * 0.5 +
-            (double)(ctx->nVBricks << (3 * ctx->grid.bshift)) * 20.0 + (double)ctx->nVBoundary * 2.0;
+  out6[5] = s4g_grid_bytes(ctx);
   return S4G_OK;
+}
+
+double s4g_grid_bytes(const s4g_ctx* ctx) {
+  const long long ntop = (long long)ctx->grid.tbx * ctx->grid.tby * ctx->grid.tbz;
+  return (double)ctx->nP * 16.0 + (double)(ctx->nCells + 1) * 4.0 + (double)ntop * 4.0 +
+         (double)ntop * 4.0 + (double)(ctx->nVBricks << (3 * ctx->grid.bshift)) * 0.5 +
+         (double)(ctx->nVBricks << (3 * ctx->grid.bshift)) * 20.0 + (double)ctx->nVBoundary * 2.0;
 }
 
 // =============================================================================================
@@ -750,6 +757,7 @@ extern "C" int s4g_set_cloud_q(s4g_ctx* ctx, const float* xyz, const float* norm
   S4G_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
   ctx->nQ = 0;
+  ctx->patch_np = 0;
   ctx->pair_index_ready = false;
   ctx->nPairs[0] = ctx->nPairs[1] = 0;
   ctx->nQuads = 0;

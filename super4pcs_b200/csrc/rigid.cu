@@ -15,8 +15,6 @@
 #include <cmath>
 #include <vector>
 
-int s4g_launch_verify(s4g_ctx* ctx, const float* d_T12, int K, uint32_t* d_counts, bool timed, const uint32_t* d_K);
-
 namespace {
 
 struct BaseArgs {
@@ -117,12 +115,12 @@ __device__ void rigid_fit(const BaseArgs& B, float3 q0, float3 q1, float3 q2, Ri
 }
 
 // mode 0: write dense outputs (T16 column-major, rms, ok) for every quad (s4g_rigid_batch)
-// mode 1: compact gate-passing candidates: T12 row-major, quad index
+// mode 1: compact gate-passing candidates: Verify record (row-major 3x4 + what Verify derives from it), quad index
 template <int kMode>
 __global__ void k_rigid(BaseArgs B, const float4* __restrict__ Q, int nQ, const int4* __restrict__ quads,
                         long long K, int shard_rank, int shard_world, float* __restrict__ outT,
                         float* __restrict__ outRms, int* __restrict__ outOk, uint32_t* __restrict__ candIdx,
-                        uint32_t* __restrict__ nCand) {
+                        uint32_t* __restrict__ nCand, VerifyRecArgs ra, VerifyCand* __restrict__ outRec) {
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   bool active = i < K;
   if (kMode == 1 && active && shard_world > 1) active = (i % shard_world) == shard_rank;
@@ -171,10 +169,9 @@ __global__ void k_rigid(BaseArgs B, const float4* __restrict__ Q, int nQ, const 
   if (pass) {
     uint32_t slot = base + __popc(b & ((1u << lane) - 1u));
     candIdx[slot] = (uint32_t)i;
-    float* T = outT + (size_t)slot * 12;
-    T[0] = r.R[0][0]; T[1] = r.R[0][1]; T[2] = r.R[0][2]; T[3] = r.t.x;
-    T[4] = r.R[1][0]; T[5] = r.R[1][1]; T[6] = r.R[1][2]; T[7] = r.t.y;
-    T[8] = r.R[2][0]; T[9] = r.R[2][1]; T[10] = r.R[2][2]; T[11] = r.t.z;
+    float m[12] = {r.R[0][0], r.R[0][1], r.R[0][2], r.t.x, r.R[1][0], r.R[1][1], r.R[1][2], r.t.y,
+                   r.R[2][0], r.R[2][1], r.R[2][2], r.t.z};
+    s4g_verify_record(m, ra, &outRec[slot]);
     outRms[slot] = r.rms;
   }
 }
@@ -214,7 +211,7 @@ __global__ void k_argmax_n(const uint32_t* __restrict__ counts, const uint32_t* 
 
 // find the compacted slot of the winner and assemble the result record
 __global__ void k_finish(const uint32_t* __restrict__ candIdx, const uint32_t* __restrict__ nCand,
-                         const float* __restrict__ T12, const float* __restrict__ rms,
+                         const VerifyCand* __restrict__ recs, const float* __restrict__ rms,
                          const unsigned long long* __restrict__ best, BaseArgs B,
                          const float4* __restrict__ Q, const int4* __restrict__ quads, int nQ,
                          s4g_tcs_result* __restrict__ out) {
@@ -238,7 +235,7 @@ __global__ void k_finish(const uint32_t* __restrict__ candIdx, const uint32_t* _
   uint32_t widx = 0xFFFFFFFFu - (uint32_t)(key & 0xFFFFFFFFull);
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     if (candIdx[i] == widx) {
-      const float* T = T12 + (size_t)i * 12;
+      const float* T = recs[i].T;
       out->best_count = (uint32_t)(key >> 32);
       out->best_index = (int32_t)widx;
       out->best_rms = rms[i];
@@ -282,9 +279,9 @@ BaseArgs make_base(const float* b, float max_angle_deg, float rms_threshold) {
 namespace {
 
 __global__ void k_brigid(const BaseArgs* __restrict__ args, const float4* __restrict__ Q, int nQ, const int4* __restrict__ quads,
-                         const unsigned long long* __restrict__ qkeys, long long K, float* __restrict__ outT,
-                         float* __restrict__ outRms, uint32_t* __restrict__ candIdx, uint32_t* __restrict__ nCand,
-                         uint32_t* __restrict__ gateCnt) {
+                         const unsigned long long* __restrict__ qkeys, long long K, VerifyRecArgs ra,
+                         VerifyCand* __restrict__ outRec, float* __restrict__ outRms, uint32_t* __restrict__ candIdx,
+                         uint32_t* __restrict__ nCand, uint32_t* __restrict__ gateCnt) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   Rigid r;
   r.ok = false;
@@ -312,10 +309,9 @@ __global__ void k_brigid(const BaseArgs* __restrict__ args, const float4* __rest
   if (pass) {
     const uint32_t slot = slot0 + __popc(b & ((1u << lane) - 1u));
     candIdx[slot] = (uint32_t)i;
-    float* T = outT + (size_t)slot * 12;
-    T[0] = r.R[0][0]; T[1] = r.R[0][1]; T[2] = r.R[0][2]; T[3] = r.t.x;
-    T[4] = r.R[1][0]; T[5] = r.R[1][1]; T[6] = r.R[1][2]; T[7] = r.t.y;
-    T[8] = r.R[2][0]; T[9] = r.R[2][1]; T[10] = r.R[2][2]; T[11] = r.t.z;
+    float m[12] = {r.R[0][0], r.R[0][1], r.R[0][2], r.t.x, r.R[1][0], r.R[1][1], r.R[1][2], r.t.y,
+                   r.R[2][0], r.R[2][1], r.R[2][2], r.t.z};
+    s4g_verify_record(m, ra, &outRec[slot]);
     outRms[slot] = r.rms;
     atomicAdd(&gateCnt[base], 1u);
   }
@@ -333,7 +329,7 @@ __global__ void k_bargmax(const uint32_t* __restrict__ counts, const uint32_t* _
 }
 
 // blockIdx.y = base
-__global__ void k_bfinish(const uint32_t* __restrict__ candIdx, const uint32_t* __restrict__ nCand, const float* __restrict__ T12,
+__global__ void k_bfinish(const uint32_t* __restrict__ candIdx, const uint32_t* __restrict__ nCand, const VerifyCand* __restrict__ recs,
                           const float* __restrict__ rms, const unsigned long long* __restrict__ best, const BaseArgs* __restrict__ args,
                           const float4* __restrict__ Q, const int4* __restrict__ quads, const uint32_t* __restrict__ quadOff,
                           const uint32_t* __restrict__ gateCnt, int nQ, s4g_base_result* __restrict__ outs) {
@@ -361,7 +357,7 @@ __global__ void k_bfinish(const uint32_t* __restrict__ candIdx, const uint32_t* 
   const uint32_t target = quadOff[base] + widx;
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     if (candIdx[i] == target) {
-      const float* T = T12 + (size_t)i * 12;
+      const float* T = recs[i].T;
       out->best_count = (uint32_t)(key >> 32);
       out->best_index = (int32_t)widx;
       out->best_rms = rms[i];
@@ -400,7 +396,7 @@ int s4g_batch_tcs(s4g_ctx* ctx, const s4g_base_desc* bases, float max_angle_deg,
   S4G_CUDA(cudaMemcpyAsync(ctx->bArgs.p, args.data(), args.size() * sizeof(BaseArgs), cudaMemcpyHostToDevice, st));
   if (K == 0) S4G_CUDA(cudaMemcpyAsync(d_quadOff, bh.quadOff, (size_t)(B + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
   const long long cap = std::max<long long>(K, 1);
-  S4G_TRY(s4g_reserve(ctx, ctx->dT12, (size_t)cap * 12 * sizeof(float)));
+  S4G_TRY(s4g_reserve(ctx, ctx->dVrec, (size_t)cap * sizeof(VerifyCand)));
   S4G_TRY(s4g_reserve(ctx, ctx->dRms, (size_t)cap * sizeof(float)));
   S4G_TRY(s4g_reserve(ctx, ctx->dCandIdx, (size_t)cap * sizeof(uint32_t)));
   S4G_TRY(s4g_reserve(ctx, ctx->dCounts, (size_t)cap * sizeof(uint32_t)));
@@ -409,22 +405,23 @@ int s4g_batch_tcs(s4g_ctx* ctx, const s4g_base_desc* bases, float max_angle_deg,
     const unsigned long long* qk = ctx->bQuadKeys[1].as<unsigned long long>();
     S4G_EV_START(ctx, S4G_EV_RIGID);
     k_brigid<<<(unsigned)((K + 127) / 128), 128, 0, st>>>(d_args, ctx->dQ.as<float4>(), ctx->nQ, ctx->bQuads.as<int4>(), qk, K,
-                                                         ctx->dT12.as<float>(), ctx->dRms.as<float>(), ctx->dCandIdx.as<uint32_t>(),
-                                                         d_nCand, d_gate);
+                                                         s4g_verify_rec_args(ctx), ctx->dVrec.as<VerifyCand>(), ctx->dRms.as<float>(),
+                                                         ctx->dCandIdx.as<uint32_t>(), d_nCand, d_gate);
     S4G_EV_STOP(ctx, S4G_EV_RIGID);
     // Verify over the compacted candidates of all bases; their number stays on the device (K quads is the upper bound)
-    if (K <= 65535ll * 16) {
-      S4G_TRY(s4g_launch_verify(ctx, ctx->dT12.as<float>(), (int)K, ctx->dCounts.as<uint32_t>(), true, d_nCand));
-    } else {                                                        // more than one grid slab: the count has to come to the host
+    if (K <= 0x7fffffffll) {
+      S4G_TRY(s4g_launch_verify(ctx, ctx->dVrec.as<VerifyCand>(), (int)K, ctx->dCounts.as<uint32_t>(), true, d_nCand));
+    } else {                                                        // beyond Verify's int K: the count has to come to the host
       uint32_t nCand = 0;
       S4G_CUDA(cudaMemcpyAsync(&nCand, d_nCand, sizeof nCand, cudaMemcpyDeviceToHost, st));
       S4G_CUDA(cudaStreamSynchronize(st));
-      S4G_TRY(s4g_launch_verify(ctx, ctx->dT12.as<float>(), (int)nCand, ctx->dCounts.as<uint32_t>(), true, nullptr));
+      if (nCand > 0x7fffffffu) { ctx->err = "s4g_try_bases: more than 2^31-1 gate-passing quads in one call"; return S4G_ERR_NOMEM; }
+      S4G_TRY(s4g_launch_verify(ctx, ctx->dVrec.as<VerifyCand>(), (int)nCand, ctx->dCounts.as<uint32_t>(), true, nullptr));
     }
     k_bargmax<<<64, 256, 0, st>>>(ctx->dCounts.as<uint32_t>(), ctx->dCandIdx.as<uint32_t>(), d_nCand, qk, d_quadOff, d_best);
     ctx->launches += 2;
   }
-  k_bfinish<<<dim3(K > 0 ? 32 : 1, (unsigned)B, 1), 256, 0, st>>>(ctx->dCandIdx.as<uint32_t>(), d_nCand, ctx->dT12.as<float>(),
+  k_bfinish<<<dim3(K > 0 ? 32 : 1, (unsigned)B, 1), 256, 0, st>>>(ctx->dCandIdx.as<uint32_t>(), d_nCand, ctx->dVrec.as<VerifyCand>(),
                                                                   ctx->dRms.as<float>(), d_best, d_args, ctx->dQ.as<float4>(),
                                                                   ctx->bQuads.as<int4>(), d_quadOff, d_gate, ctx->nQ,
                                                                   ctx->bResults.as<s4g_base_result>());
@@ -474,7 +471,7 @@ extern "C" int s4g_rigid_batch(s4g_ctx* ctx, const float* base_xyz, const int32_
   S4G_EV_START(ctx, S4G_EV_RIGID);
   k_rigid<0><<<(unsigned)((K + 127) / 128), 128, 0, st>>>(B, ctx->dQ.as<float4>(), ctx->nQ, ctx->dScratchA.as<int4>(), K,
                                                          0, 1, ctx->dScratchB.as<float>(), ctx->dRms.as<float>(),
-                                                         ctx->dOk.as<int>(), nullptr, nullptr);
+                                                         ctx->dOk.as<int>(), nullptr, nullptr, VerifyRecArgs{}, nullptr);
   S4G_EV_STOP(ctx, S4G_EV_RIGID);
   ctx->launches++;
   S4G_CUDA(cudaGetLastError());
@@ -506,7 +503,7 @@ extern "C" int s4g_try_congruent_set_dev(s4g_ctx* ctx, const float* base_xyz, co
   BaseArgs B = make_base(base_xyz, max_angle_deg, rms_threshold);
   long long cap = shard_world > 1 ? (K + shard_world - 1) / shard_world : K;
   if (cap < 1) cap = 1;
-  S4G_TRY(s4g_reserve(ctx, ctx->dT12, (size_t)cap * 12 * sizeof(float)));
+  S4G_TRY(s4g_reserve(ctx, ctx->dVrec, (size_t)cap * sizeof(VerifyCand)));
   S4G_TRY(s4g_reserve(ctx, ctx->dRms, (size_t)cap * sizeof(float)));
   S4G_TRY(s4g_reserve(ctx, ctx->dCandIdx, (size_t)cap * sizeof(uint32_t)));
   S4G_TRY(s4g_reserve(ctx, ctx->dCounts, (size_t)cap * sizeof(uint32_t)));
@@ -521,24 +518,25 @@ extern "C" int s4g_try_congruent_set_dev(s4g_ctx* ctx, const float* base_xyz, co
     S4G_EV_START(ctx, S4G_EV_RIGID);
     k_rigid<1><<<(unsigned)((K + 127) / 128), 128, 0, st>>>(B, ctx->dQ.as<float4>(), ctx->nQ,
                                                            reinterpret_cast<const int4*>(d_quads), K, shard_rank,
-                                                           shard_world, ctx->dT12.as<float>(), ctx->dRms.as<float>(),
-                                                           nullptr, ctx->dCandIdx.as<uint32_t>(), d_nCand);
+                                                           shard_world, nullptr, ctx->dRms.as<float>(), nullptr,
+                                                           ctx->dCandIdx.as<uint32_t>(), d_nCand, s4g_verify_rec_args(ctx),
+                                                           ctx->dVrec.as<VerifyCand>());
     S4G_EV_STOP(ctx, S4G_EV_RIGID);
     ctx->launches++;
     // the candidate count sizes the Verify grid: one 4-byte readback
     S4G_CUDA(cudaMemcpyAsync(&nCand, d_nCand, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     S4G_CUDA(cudaStreamSynchronize(st));
   }
-  if (nCand > 0x7fffffffu) {  // s4g_verify* take `int K`; 2^31 transforms would be 103 GB of T12 anyway
+  if (nCand > 0x7fffffffu) {  // s4g_verify* take `int K`; 2^31 records would be 240 GB anyway
     ctx->err = "s4g_try_congruent_set: more than 2^31-1 gate-passing quads in one call (shard the set)";
     return S4G_ERR_NOMEM;
   }
   if (nCand > 0) {
-    S4G_TRY(s4g_launch_verify(ctx, ctx->dT12.as<float>(), (int)nCand, ctx->dCounts.as<uint32_t>(), true, nullptr));
+    S4G_TRY(s4g_launch_verify(ctx, ctx->dVrec.as<VerifyCand>(), (int)nCand, ctx->dCounts.as<uint32_t>(), true, nullptr));
     k_argmax<<<64, 256, 0, st>>>(ctx->dCounts.as<uint32_t>(), ctx->dCandIdx.as<uint32_t>(), d_nCand, d_best);
     ctx->launches++;
   }
-  k_finish<<<64, 256, 0, st>>>(ctx->dCandIdx.as<uint32_t>(), d_nCand, ctx->dT12.as<float>(), ctx->dRms.as<float>(),
+  k_finish<<<64, 256, 0, st>>>(ctx->dCandIdx.as<uint32_t>(), d_nCand, ctx->dVrec.as<VerifyCand>(), ctx->dRms.as<float>(),
                                d_best, B, ctx->dQ.as<float4>(), reinterpret_cast<const int4*>(d_quads), ctx->nQ,
                                ctx->dResult.as<s4g_tcs_result>());
   ctx->launches++;

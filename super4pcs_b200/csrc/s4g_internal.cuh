@@ -73,6 +73,7 @@ struct s4g_ctx {
   cudaStream_t own_stream = nullptr;
   std::string err;
   int sm_count = 132;
+  long long l2_bytes = 50ll << 20;   // the device's L2 (sizes the query patches of Verify)
 
   // ---- P side
   int nP = 0;
@@ -93,6 +94,8 @@ struct s4g_ctx {
   DevBuf dQmside;   // Morton-ordered copies of unit coordinates | normals | rgb (3 x n float4) for the pair predicate
   DevBuf dQtiles;   // bounding spheres (centre, radius): [nTiles] of every kVerifyTile consecutive Morton points, then [nSubs] of every kVerifySub
   DevBuf dQgroups;  // AABBs of the 64-point groups / 64-group supergroups of the Morton order
+  DevBuf dQpatch;   // centres (float4) of Verify's query patches: runs of patch_tiles consecutive super-tiles (verify.cu)
+  int patch_np = 0, patch_tiles = 0;   // patch count and length the centres were computed for (0: none yet)
   bool pair_index_ready = false;
   bool q_has_normals = false, q_has_rgb = false;
   float qabs[3] = {0, 0, 0};   // largest |coordinate| of sampled Q per axis (rounding bound of the cell-space transform)
@@ -111,7 +114,8 @@ struct s4g_ctx {
 
   // ---- scratch
   DevBuf dScratchA, dScratchB, dScratchC, dScratchD, dCub;
-  DevBuf dT12, dRms, dOk, dCandIdx, dCounts, dResult, dMisc;
+  DevBuf dRms, dOk, dCandIdx, dCounts, dResult, dMisc;
+  DevBuf dVrec, dVsort;   // Verify: per-candidate records; per-patch candidate order (sort keys, values, CUB temp)
   void* hPinned = nullptr;  // small pinned staging block
   size_t hPinnedBytes = 0;
 
@@ -136,6 +140,8 @@ constexpr int kVerifyTile = 128;
 constexpr int kVerifySub = 32;
 
 int s4g_reserve(s4g_ctx* ctx, DevBuf& b, size_t bytes);
+// device bytes of the sorted P, its grid and the delta-field (what Verify looks up besides Q)
+double s4g_grid_bytes(const s4g_ctx* ctx);
 
 // comm.cu: the reduction of the shards' winners on the device (active when a communicator is attached and shard_world > 1)
 bool s4g_comm_active(const s4g_ctx* ctx, int shard_world);
@@ -206,3 +212,50 @@ __device__ __forceinline__ float3 s4_normalized(float3 a) {
   return a;
 }
 __device__ __forceinline__ float3 s4_xyz(float4 v) { return make_float3(v.x, v.y, v.z); }
+
+// ---- Verify's candidate records (verify.cu), written by whatever produces the candidates (k_pack_rec for the API
+// entry points, the rigid fits of rigid.cu), so that Verify needs no launch of its own to derive them
+struct __align__(16) VerifyCand {
+  float T[12];     // exact 3x4, row-major (r00 r01 r02 t0 | r10 ...): the top three rows of T (decision arithmetic)
+  float V[12];     // voxel-space 3x4 V = S T (selection only)
+  float scale;     // tile-cull radius scale (>= the operator norm of T's 3x3 part); < 0: robust path, no cull
+  float pad[3];
+};
+// what a record depends on besides T: the grid's origin and voxel scale, the delta-field's margin, max |q| per axis of Q
+struct VerifyRecArgs {
+  float ox, oy, oz, inv_v, vslack, qax, qay, qaz;
+};
+inline VerifyRecArgs s4g_verify_rec_args(const s4g_ctx* ctx) {
+  return VerifyRecArgs{ctx->grid.ox, ctx->grid.oy, ctx->grid.oz, ctx->grid.inv_v, ctx->grid.vslack,
+                       ctx->qabs[0], ctx->qabs[1], ctx->qabs[2]};
+}
+__device__ __forceinline__ void s4g_verify_record(const float (&m)[12], const VerifyRecArgs& a, VerifyCand* __restrict__ out) {
+  VerifyCand r;
+#pragma unroll
+  for (int i = 0; i < 12; ++i) {
+    const int col = i & 3, row = i >> 2;
+    const float o = row == 0 ? a.ox : row == 1 ? a.oy : a.oz;
+    r.T[i] = m[i];
+    r.V[i] = col < 3 ? m[i] * a.inv_v : (m[i] - o) * a.inv_v;
+  }
+  // rounding bound of this candidate's voxel position (fast path) against the margin the field was built with:
+  // |x~ - fl(T q)| <= 2^-20 max_r (sum_j |T_rj| |q_j| + |T_r3| + |o_r|)   (16 roundings of relative size 2^-24)
+  const float w0 = fabsf(m[0]) * a.qax + fabsf(m[1]) * a.qay + fabsf(m[2]) * a.qaz + fabsf(m[3]) + fabsf(a.ox);
+  const float w1 = fabsf(m[4]) * a.qax + fabsf(m[5]) * a.qay + fabsf(m[6]) * a.qaz + fabsf(m[7]) + fabsf(a.oy);
+  const float w2 = fabsf(m[8]) * a.qax + fabsf(m[9]) * a.qay + fabsf(m[10]) * a.qaz + fabsf(m[11]) + fabsf(a.oz);
+  const float E = fmaxf(w0, fmaxf(w1, w2)) * 9.5367431640625e-7f;   // 2^-20
+  // operator norm of the 3x3 part: ||A||_2^2 = lambda_max(A^T A) <= max row sum of |A^T A| (= 1 for a rotation)
+  const float g00 = m[0] * m[0] + m[4] * m[4] + m[8] * m[8], g11 = m[1] * m[1] + m[5] * m[5] + m[9] * m[9],
+              g22 = m[2] * m[2] + m[6] * m[6] + m[10] * m[10];
+  const float g01 = fabsf(m[0] * m[1] + m[4] * m[5] + m[8] * m[9]), g02 = fabsf(m[0] * m[2] + m[4] * m[6] + m[8] * m[10]),
+              g12 = fabsf(m[1] * m[2] + m[5] * m[6] + m[9] * m[10]);
+  const float n2 = fmaxf(g00 + g01 + g02, fmaxf(g01 + g11 + g12, g02 + g12 + g22));
+  const float s = sqrtf(n2) * 1.00001f;
+  const bool precise = (E <= a.vslack) && (s <= 1.0e6f);     // false for NaN / Inf
+  r.scale = precise ? s : -1.f;
+  r.pad[0] = r.pad[1] = r.pad[2] = 0.f;
+  *out = r;
+}
+// Enqueue Verify of K candidate records (device); zeroes d_counts first.  d_K: the candidate count when only the device
+// knows it (K is then its upper bound)
+int s4g_launch_verify(s4g_ctx* ctx, const VerifyCand* d_recs, int K, uint32_t* d_counts, bool timed, const uint32_t* d_K);
