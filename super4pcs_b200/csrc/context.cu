@@ -97,6 +97,8 @@ extern "C" int s4g_create(int device, s4g_ctx** out_ctx) {
     ctx->sm_count = prop.multiProcessorCount;
     if (prop.l2CacheSize > 0) ctx->l2_bytes = prop.l2CacheSize;
   }
+  // A/B knob: a fixed number of query patches for Verify instead of the one derived from the L2 size (verify.cu)
+  if (const char* e = std::getenv("S4G_VERIFY_PATCHES")) ctx->verify_patches = std::max(0, std::min(kVerifyMaxPatches, std::atoi(e)));
   {
     // keep freed scratch in the pool instead of returning it to the driver at every synchronisation
     cudaMemPool_t pool = nullptr;

@@ -96,6 +96,7 @@ struct s4g_ctx {
   DevBuf dQgroups;  // AABBs of the 64-point groups / 64-group supergroups of the Morton order
   DevBuf dQpatch;   // centres (float4) of Verify's query patches: runs of patch_tiles consecutive super-tiles (verify.cu)
   int patch_np = 0, patch_tiles = 0;   // patch count and length the centres were computed for (0: none yet)
+  int verify_patches = 0;   // requested patch count (S4G_VERIFY_PATCHES when the context was created); 0: from the L2 size
   bool pair_index_ready = false;
   bool q_has_normals = false, q_has_rgb = false;
   float qabs[3] = {0, 0, 0};   // largest |coordinate| of sampled Q per axis (rounding bound of the cell-space transform)
@@ -138,6 +139,8 @@ struct s4g_ctx {
 constexpr int kVerifyTile = 128;
 // queries per cull unit (= one warp of a Verify CTA); s4g_set_cloud_q pre-computes one bounding sphere per unit
 constexpr int kVerifySub = 32;
+// most query patches of one Verify launch (verify.cu, choose_patches): the sort's scratch is 24 bytes per (patch, candidate)
+constexpr int kVerifyMaxPatches = 16;
 
 int s4g_reserve(s4g_ctx* ctx, DevBuf& b, size_t bytes);
 // device bytes of the sorted P, its grid and the delta-field (what Verify looks up besides Q)

@@ -404,13 +404,16 @@ k_verify(GridDev g, const float4* __restrict__ Q, const float4* __restrict__ til
       }
     } else {
       // robust loop (a live candidate failed the bound: huge / non-rigid / NaN coefficients): voxel from the reference-order
-      // T q, float range test (NaN and out-of-range coordinates fail it before any int conversion is used)
+      // T q, float range test (NaN and out-of-range coordinates fail it before any int conversion is used).  The other
+      // candidates keep the voxel of the fast loop (for finite coordinates its range test is the same), so the path of a
+      // (query, candidate) pair -- and with it the probe statistics -- does not depend on which candidates share its chunk.
 #pragma unroll 1
       while (live_mask) {
         const int c = __ffs(live_mask) - 1;
         live_mask &= live_mask - 1;
         float ux, uy, uz;
-        voxel_of<true>(g, &sV[c * 12], &sT[c * 12], q, ux, uy, uz);
+        if ((imprec >> c) & 1u) voxel_of<true>(g, &sV[c * 12], &sT[c * 12], q, ux, uy, uz);
+        else voxel_of<false>(g, &sV[c * 12], nullptr, q, ux, uy, uz);
         const bool in = valid && ux >= 0.f && uy >= 0.f && uz >= 0.f && ux < (float)limX && uy < (float)limY && uz < (float)limZ;
         const int X = in ? __float2int_rd(ux) : 0, Y = in ? __float2int_rd(uy) : 0, Z = in ? __float2int_rd(uz) : 0;
         const int r = in ? __ldg(&g.vtop[vtop_index<kBS>(g, X, Y, Z)]) : -1;
@@ -572,14 +575,12 @@ __global__ void k_patch_centres(const float4* __restrict__ tiles, int nTiles, in
 // Query patches (see k_verify): as many as it takes for one patch's queries and the part of the grid and delta-field its
 // images touch to fit in half of the L2 (that part is taken to be the patch's share of the whole grid); one patch when
 // everything fits.  On the H100 at 1M points this gives 5 patches; 8 and 16 measured the same within noise, 2 and 1 slower
-// (DESIGN.md section 9).  At most kMaxPatches: the sort's scratch is 24 bytes per (patch, candidate) pair.
-// S4G_VERIFY_PATCHES > 0 fixes the count instead (A/B runs).
-#ifndef S4G_VERIFY_PATCHES
-#define S4G_VERIFY_PATCHES 0
-#endif
-constexpr int kMaxPatches = 16;
+// (DESIGN.md section 9).  At most kVerifyMaxPatches: the sort's scratch is 24 bytes per (patch, candidate) pair.
+// ctx->verify_patches > 0 (the environment variable S4G_VERIFY_PATCHES when the context was created) requests the count
+// instead, for A/B runs and tests; it is capped the same way.
+constexpr int kMaxPatches = kVerifyMaxPatches;
 void choose_patches(const s4g_ctx* ctx, int nST, int& NP, int& ptiles) {
-  long long np = S4G_VERIFY_PATCHES;
+  long long np = ctx->verify_patches;
   if (np <= 0) {
     const double ws = (double)ctx->nQ * sizeof(float4) + s4g_grid_bytes(ctx);
     np = (long long)std::ceil(2.0 * ws / (double)ctx->l2_bytes);

@@ -64,6 +64,20 @@ def run(which, libpath):
                         [int(x) for x in ids]])
         out = dict(log=log)
         m.close()
+    elif which == "patches":
+        # a sampled Q of 3500 points = 4 of Verify's 1024-query super-tiles (S4G_VERIFY_PATCHES > 1 splits them into
+        # patches; s4g_try_bases is on by default at this size): 9 bases in four stepwise calls, a few seconds on the CPU
+        # (the whole run would try 72 bases, some with 80K candidates)
+        from super4pcs_b200 import synth
+        d = synth.make_pair(12000, 0.8, seed=4)
+        opt = oref.make_options(delta=0.007, overlap=0.8, sample_size=3500, random_seed=21, max_time_seconds=10000)
+        m = oref.RefMatcher(d["P"], d["Q"], opt, identity_sampler=False, libpath=libpath)
+        log = [m.nQ, _h(m.sampled_q()[0])]
+        for n in (2, 2, 3, 2):
+            r = m.perform_n_steps(n)
+            log.append([r["ret"], float(np.float32(r["best_lcp"])), r["n_progress"], [int(x) for x in r["T"].view(np.uint32)]])
+        out = dict(log=log)
+        m.close()
     elif which.startswith("synth"):
         # whole pipeline on a synthetic pair: voxel sampler, shuffle + truncation, RNG-driven bases, filters
         from super4pcs_b200 import synth

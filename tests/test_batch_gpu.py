@@ -32,10 +32,19 @@ def _bases(P, Pn, rng, k, diameter):
     return out
 
 
-@pytest.mark.parametrize("n,ns,delta,normals,nb", [(20000, 400, 0.02, False, 7), (50000, 3000, 0.01, False, 5),
-                                                   (30000, 2000, 0.015, True, 9), (5000, 70, 0.05, False, 33)])
-def test_try_bases_equals_the_per_base_chain(s4g_lib, n, ns, delta, normals, nb):
+@pytest.mark.parametrize("n,ns,delta,normals,nb,patches", [
+    pytest.param(20000, 400, 0.02, False, 7, None, id="20000-400-0.02-False-7"),
+    pytest.param(50000, 3000, 0.01, False, 5, None, id="50000-3000-0.01-False-5"),
+    pytest.param(30000, 2000, 0.015, True, 9, None, id="30000-2000-0.015-True-9"),
+    pytest.param(5000, 70, 0.05, False, 33, None, id="5000-70-0.05-False-33"),
+    # Verify's queries in 3 / 2 patches (S4G_VERIFY_PATCHES): the batched chain runs them with its device-side candidate
+    # count and candidates beyond it keyed last, the per-base chain with a host count
+    pytest.param(50000, 3000, 0.01, False, 5, 3, id="50000-3000-0.01-False-5-patches3"),
+    pytest.param(30000, 2000, 0.015, True, 9, 2, id="30000-2000-0.015-True-9-patches2")])
+def test_try_bases_equals_the_per_base_chain(s4g_lib, monkeypatch, n, ns, delta, normals, nb, patches):
     from super4pcs_b200 import Context, PairFilters
+    if patches is not None:
+        monkeypatch.setenv("S4G_VERIFY_PATCHES", str(patches))
     sc = common.scenario(n, 0.5, delta, seed=n % 97, normals=normals)
     rng = np.random.RandomState(ns)
     sel = rng.choice(n, ns, replace=False)

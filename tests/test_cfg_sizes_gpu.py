@@ -24,9 +24,12 @@ def cfg3():
     return d, P, Q
 
 
-@pytest.mark.parametrize("ns", [3000, 10000])
-def test_cfg3_base_matches_oracle(s4g_lib, cfg3, ns):
+@pytest.mark.parametrize("ns,patches", [pytest.param(3000, None, id="3000"), pytest.param(10000, None, id="10000"),
+                                        pytest.param(10000, 10, id="10000-patches10")])   # one super-tile per Verify patch
+def test_cfg3_base_matches_oracle(s4g_lib, monkeypatch, cfg3, ns, patches):
     from super4pcs_b200 import Context, PairFilters
+    if patches is not None:
+        monkeypatch.setenv("S4G_VERIFY_PATCHES", str(patches))
     d, P, Q = cfg3
     delta = 0.01
     rng = np.random.RandomState(ns)
