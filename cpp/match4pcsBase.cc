@@ -11,6 +11,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
+#include <cstring>
 #include <limits>
 #include <stdexcept>
 #include <string>
@@ -478,17 +479,20 @@ void Match4PCSBase::DeviceTryCongruentSet(const int base_ids[4], const std::vect
                               &shard[size_t(rank)]) != S4G_OK)
       ThrowLaneError(ctx, "s4g_try_congruent_set");
   });
-  const s4g_tcs_result r = detail::CombineShards(shard, nccl_);
-  out->any = r.best_index >= 0;
-  out->count = r.best_count;
-  out->n_q = r.n_q ? r.n_q : 1;
-  out->index = r.best_index;
-  out->n_gate_pass = r.n_gate_pass;
-  if (out->any) {
-    for (int k = 0; k < 4; ++k) out->quad[k] = quads[size_t(r.best_index)].vertices[k];
-    out->T = Eigen::Map<const MatrixType>(r.best_T);
-    out->centroid1 = Eigen::Map<const VectorType>(r.centroid1);
-    out->centroid2 = Eigen::Map<const VectorType>(r.centroid2);
+  out->SetFrom(detail::CombineShards(shard, nccl_));
+}
+
+void Match4PCSBase::DeviceBest::SetFrom(const s4g_tcs_result& r) {
+  any = r.best_index >= 0;
+  count = r.best_count;
+  n_q = r.n_q ? r.n_q : 1;
+  index = r.best_index;
+  n_gate_pass = r.n_gate_pass;
+  if (any) {
+    std::memcpy(quad, r.best_quad, sizeof r.best_quad);
+    T = Eigen::Map<const MatrixType>(r.best_T);
+    centroid1 = Eigen::Map<const VectorType>(r.centroid1);
+    centroid2 = Eigen::Map<const VectorType>(r.centroid2);
   }
 }
 

@@ -243,18 +243,7 @@ bool MatchSuper4PCS::TryBaseOnLane(s4g_ctx* lane, const std::vector<Point3D>& ba
   if (pass[0].nq == 0) return true;
   std::vector<s4g_tcs_result> shard;
   for (const Pass& p : pass) shard.push_back(p.r);
-  const s4g_tcs_result r = detail::CombineShards(shard, nccl_);
-  out->any = r.best_index >= 0;
-  out->count = r.best_count;
-  out->n_q = r.n_q ? r.n_q : 1;
-  out->index = r.best_index;
-  out->n_gate_pass = r.n_gate_pass;
-  if (out->any) {
-    std::memcpy(out->quad, r.best_quad, sizeof r.best_quad);
-    out->T = Eigen::Map<const MatrixType>(r.best_T);
-    out->centroid1 = Eigen::Map<const VectorType>(r.centroid1);
-    out->centroid2 = Eigen::Map<const VectorType>(r.centroid2);
-  }
+  out->SetFrom(detail::CombineShards(shard, nccl_));
   return true;
 }
 
@@ -293,17 +282,7 @@ bool MatchSuper4PCS::TryBasesOnLane(s4g_ctx* lane, const std::vector<Speculative
     out.n_pairs[0] = long(r.n_pairs[0]);
     out.n_pairs[1] = long(r.n_pairs[1]);
     out.n_quads = long(r.n_quads);
-    out.any = r.tcs.best_index >= 0;
-    out.count = r.tcs.best_count;
-    out.n_q = r.tcs.n_q ? r.tcs.n_q : 1;
-    out.index = r.tcs.best_index;
-    out.n_gate_pass = r.tcs.n_gate_pass;
-    if (out.any) {
-      std::memcpy(out.quad, r.tcs.best_quad, sizeof r.tcs.best_quad);
-      out.T = Eigen::Map<const MatrixType>(r.tcs.best_T);
-      out.centroid1 = Eigen::Map<const VectorType>(r.tcs.centroid1);
-      out.centroid2 = Eigen::Map<const VectorType>(r.tcs.centroid2);
-    }
+    out.SetFrom(r.tcs);
     sb.lane = lane;
     sb.handled = true;
     sb.batched = true;

@@ -30,6 +30,7 @@
 #include "super4pcs/utils/logger.h"
 
 struct s4g_ctx;  // include/s4g.h (opaque here: callers need no CUDA headers)
+struct s4g_tcs_result;
 
 namespace GlobalRegistration {
 
@@ -155,6 +156,8 @@ class Match4PCSBase {
     double stage_ms[4] = {0, 0, 0, 0};  ///< S4PCS_TIMINGS: device ms of pairs (both calls) / quads / rigid fit / Verify
     Eigen::Matrix<Scalar, 4, 4, Eigen::DontAlign> T;  ///< (unaligned: lives in std containers)
     VectorType centroid1, centroid2;
+    /// the winner and the counts of a TryCongruentSet result record; the pair / quad counts and stage times stay as they are
+    void SetFrom(const s4g_tcs_result& r);
   };
   /// One fused pass pairs -> quads -> rigid fit -> Verify entirely on the device.  The base
   /// implementation reports "unsupported" (returns false) so that subclasses providing only

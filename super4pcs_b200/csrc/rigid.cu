@@ -114,8 +114,48 @@ __device__ void rigid_fit(const BaseArgs& B, float3 q0, float3 q1, float3 q2, Ri
   o.t = s4_add(B.c1, mulMV(o.R, make_float3(-o.c2.x, -o.c2.y, -o.c2.z)));
 }
 
+// rigid fit of quad qd; returns whether it passes the gate.  A quad with an index outside sampled Q is not fitted
+// (r.ok == false, r.rms == -1).
+__device__ __forceinline__ bool fit_quad(const BaseArgs& B, const float4* __restrict__ Q, int nQ, int4 qd, Rigid& r) {
+  r.ok = false;
+  r.rms = -1.f;
+  bool inb = (unsigned)qd.x < (unsigned)nQ && (unsigned)qd.y < (unsigned)nQ && (unsigned)qd.z < (unsigned)nQ &&
+             (unsigned)qd.w < (unsigned)nQ;
+  if (!inb) return false;
+  float3 q0 = s4_xyz(__ldg(&Q[qd.x])), q1 = s4_xyz(__ldg(&Q[qd.y])), q2 = s4_xyz(__ldg(&Q[qd.z]));
+  rigid_fit(B, q0, q1, q2, r);
+  return r.ok && r.rms >= 0.f && r.rms < B.rms_threshold;  // hpp:436-439
+}
+
+// warp-aggregated append of the warp's gate-passing candidates (every lane calls it): quad index i, the Verify record
+// (row-major 3x4 + what Verify derives from it) and the rms go to the next free slots of the compacted list
+__device__ __forceinline__ void append_candidate(bool pass, uint32_t i, const Rigid& r, const VerifyRecArgs& ra,
+                                                 uint32_t* __restrict__ nCand, uint32_t* __restrict__ candIdx,
+                                                 VerifyCand* __restrict__ outRec, float* __restrict__ outRms) {
+  unsigned b = __ballot_sync(0xffffffffu, pass);
+  if (b == 0u) return;
+  int lane = threadIdx.x & 31;
+  int leader = __ffs(b) - 1;
+  uint32_t base = 0;
+  if (lane == leader) base = atomicAdd(nCand, (uint32_t)__popc(b));
+  base = __shfl_sync(0xffffffffu, base, leader);
+  if (pass) {
+    uint32_t slot = base + __popc(b & ((1u << lane) - 1u));
+    candIdx[slot] = i;
+    float m[12] = {r.R[0][0], r.R[0][1], r.R[0][2], r.t.x, r.R[1][0], r.R[1][1], r.R[1][2], r.t.y,
+                   r.R[2][0], r.R[2][1], r.R[2][2], r.t.z};
+    s4g_verify_record(m, ra, &outRec[slot]);
+    outRms[slot] = r.rms;
+  }
+}
+
+// packed arg-max key of a verified candidate (see the top of this file)
+__device__ __forceinline__ unsigned long long cand_key(uint32_t count, uint32_t index) {
+  return ((unsigned long long)count << 32) | (unsigned long long)(0xFFFFFFFFu - index);
+}
+
 // mode 0: write dense outputs (T16 column-major, rms, ok) for every quad (s4g_rigid_batch)
-// mode 1: compact gate-passing candidates: Verify record (row-major 3x4 + what Verify derives from it), quad index
+// mode 1: compact gate-passing candidates (append_candidate)
 template <int kMode>
 __global__ void k_rigid(BaseArgs B, const float4* __restrict__ Q, int nQ, const int4* __restrict__ quads,
                         long long K, int shard_rank, int shard_world, float* __restrict__ outT,
@@ -125,19 +165,7 @@ __global__ void k_rigid(BaseArgs B, const float4* __restrict__ Q, int nQ, const 
   bool active = i < K;
   if (kMode == 1 && active && shard_world > 1) active = (i % shard_world) == shard_rank;
   Rigid r;
-  r.ok = false;
-  r.rms = -1.f;
-  bool pass = false;
-  if (active) {
-    int4 qd = quads[i];
-    bool inb = (unsigned)qd.x < (unsigned)nQ && (unsigned)qd.y < (unsigned)nQ && (unsigned)qd.z < (unsigned)nQ &&
-               (unsigned)qd.w < (unsigned)nQ;
-    if (inb) {
-      float3 q0 = s4_xyz(__ldg(&Q[qd.x])), q1 = s4_xyz(__ldg(&Q[qd.y])), q2 = s4_xyz(__ldg(&Q[qd.z]));
-      rigid_fit(B, q0, q1, q2, r);
-      pass = r.ok && r.rms >= 0.f && r.rms < B.rms_threshold;  // hpp:436-439
-    }
-  }
+  bool pass = active && fit_quad(B, Q, nQ, quads[i], r);
   if (kMode == 0) {
     if (!active) return;
     float* T = outT ? outT + i * 16 : nullptr;
@@ -158,31 +186,16 @@ __global__ void k_rigid(BaseArgs B, const float4* __restrict__ Q, int nQ, const 
     if (outOk) outOk[i] = r.ok ? 1 : 0;
     return;
   }
-  // warp-aggregated append
-  unsigned b = __ballot_sync(0xffffffffu, pass);
-  if (b == 0u) return;
-  int lane = threadIdx.x & 31;
-  int leader = __ffs(b) - 1;
-  uint32_t base = 0;
-  if (lane == leader) base = atomicAdd(nCand, (uint32_t)__popc(b));
-  base = __shfl_sync(0xffffffffu, base, leader);
-  if (pass) {
-    uint32_t slot = base + __popc(b & ((1u << lane) - 1u));
-    candIdx[slot] = (uint32_t)i;
-    float m[12] = {r.R[0][0], r.R[0][1], r.R[0][2], r.t.x, r.R[1][0], r.R[1][1], r.R[1][2], r.t.y,
-                   r.R[2][0], r.R[2][1], r.R[2][2], r.t.z};
-    s4g_verify_record(m, ra, &outRec[slot]);
-    outRms[slot] = r.rms;
-  }
+  append_candidate(pass, (uint32_t)i, r, ra, nCand, candIdx, outRec, outRms);
 }
 
-// packed-key arg-max over the verified candidates
-__global__ void k_argmax(const uint32_t* __restrict__ counts, const uint32_t* __restrict__ candIdx,
-                         const uint32_t* __restrict__ nCand, unsigned long long* __restrict__ best) {
-  uint32_t n = *nCand;
+// packed-key arg-max over n verified candidates (*nCand when given); the key's index is index[i] (nullptr: i)
+__global__ void k_argmax(const uint32_t* __restrict__ counts, const uint32_t* __restrict__ index,
+                         const uint32_t* __restrict__ nCand, uint32_t n, unsigned long long* __restrict__ best) {
+  if (nCand) n = *nCand;
   unsigned long long key = 0;
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    unsigned long long k = ((unsigned long long)counts[i] << 32) | (unsigned long long)(0xFFFFFFFFu - candIdx[i]);
+    unsigned long long k = cand_key(counts[i], index ? index[i] : i);
     key = k > key ? k : key;
   }
 #pragma unroll
@@ -193,33 +206,17 @@ __global__ void k_argmax(const uint32_t* __restrict__ counts, const uint32_t* __
   if ((threadIdx.x & 31) == 0 && key) atomicMax(best, key);
 }
 
-// same for a plain candidate list: n counts, index[i] = position in the caller's whole list (nullptr: i)
-__global__ void k_argmax_n(const uint32_t* __restrict__ counts, const uint32_t* __restrict__ index, uint32_t n,
-                           unsigned long long* __restrict__ best) {
-  unsigned long long key = 0;
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    unsigned long long k = ((unsigned long long)counts[i] << 32) | (unsigned long long)(0xFFFFFFFFu - (index ? index[i] : i));
-    key = k > key ? k : key;
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    unsigned long long other = __shfl_xor_sync(0xffffffffu, key, o);
-    key = other > key ? other : key;
-  }
-  if ((threadIdx.x & 31) == 0 && key) atomicMax(best, key);
-}
-
-// find the compacted slot of the winner and assemble the result record
-__global__ void k_finish(const uint32_t* __restrict__ candIdx, const uint32_t* __restrict__ nCand,
-                         const VerifyCand* __restrict__ recs, const float* __restrict__ rms,
-                         const unsigned long long* __restrict__ best, BaseArgs B,
-                         const float4* __restrict__ Q, const int4* __restrict__ quads, int nQ,
-                         s4g_tcs_result* __restrict__ out) {
-  uint32_t n = *nCand;
-  unsigned long long key = *best;
+// the result record of one congruent set from its arg-max key: the candidates are candIdx[0, n) (with their Verify
+// records and rms), the key's quad index counts from quads[quadOff], gate = the set's gate-passing candidates.
+// Grid-stride over the candidates: the thread that holds the winner writes its part.
+__device__ __forceinline__ void write_result(unsigned long long key, uint32_t gate, int nQ, const BaseArgs& B,
+                                             const uint32_t* __restrict__ candIdx, uint32_t n,
+                                             const VerifyCand* __restrict__ recs, const float* __restrict__ rms,
+                                             const float4* __restrict__ Q, const int4* __restrict__ quads,
+                                             uint32_t quadOff, s4g_tcs_result* __restrict__ out) {
   if (blockIdx.x == 0 && threadIdx.x == 0) {
     out->key = key;
-    out->n_gate_pass = n;
+    out->n_gate_pass = gate;
     out->n_q = (uint32_t)nQ;
     out->centroid1[0] = B.c1.x; out->centroid1[1] = B.c1.y; out->centroid1[2] = B.c1.z;
     if (key == 0ull) {
@@ -232,9 +229,10 @@ __global__ void k_finish(const uint32_t* __restrict__ candIdx, const uint32_t* _
     }
   }
   if (key == 0ull) return;
-  uint32_t widx = 0xFFFFFFFFu - (uint32_t)(key & 0xFFFFFFFFull);
+  const uint32_t widx = 0xFFFFFFFFu - (uint32_t)(key & 0xFFFFFFFFull);
+  const uint32_t target = quadOff + widx;
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    if (candIdx[i] == widx) {
+    if (candIdx[i] == target) {
       const float* T = recs[i].T;
       out->best_count = (uint32_t)(key >> 32);
       out->best_index = (int32_t)widx;
@@ -244,12 +242,22 @@ __global__ void k_finish(const uint32_t* __restrict__ candIdx, const uint32_t* _
         for (int c = 0; c < 4; ++c) out->best_T[4 * c + r] = T[4 * r + c];
       out->best_T[3] = out->best_T[7] = out->best_T[11] = 0.f;
       out->best_T[15] = 1.f;
-      int4 qd = quads[widx];
+      const int4 qd = quads[target];
       float3 c2 = s4_div(s4_add(s4_add(s4_xyz(Q[qd.x]), s4_xyz(Q[qd.y])), s4_xyz(Q[qd.z])), 3.f);
       out->centroid2[0] = c2.x; out->centroid2[1] = c2.y; out->centroid2[2] = c2.z;
       out->best_quad[0] = qd.x; out->best_quad[1] = qd.y; out->best_quad[2] = qd.z; out->best_quad[3] = qd.w;
     }
   }
+}
+
+// find the compacted slot of the winner and assemble the result record
+__global__ void k_finish(const uint32_t* __restrict__ candIdx, const uint32_t* __restrict__ nCand,
+                         const VerifyCand* __restrict__ recs, const float* __restrict__ rms,
+                         const unsigned long long* __restrict__ best, BaseArgs B,
+                         const float4* __restrict__ Q, const int4* __restrict__ quads, int nQ,
+                         s4g_tcs_result* __restrict__ out) {
+  const uint32_t n = *nCand;
+  write_result(*best, n, nQ, B, candIdx, n, recs, rms, Q, quads, 0u, out);
 }
 
 BaseArgs make_base(const float* b, float max_angle_deg, float rms_threshold) {
@@ -284,37 +292,14 @@ __global__ void k_brigid(const BaseArgs* __restrict__ args, const float4* __rest
                          uint32_t* __restrict__ nCand, uint32_t* __restrict__ gateCnt) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   Rigid r;
-  r.ok = false;
-  r.rms = -1.f;
   bool pass = false;
   uint32_t base = 0;
   if (i < K) {
     base = (uint32_t)(qkeys[i] >> kBatchSegShift);
-    const BaseArgs B = args[base];
-    const int4 qd = quads[i];
-    const bool inb = (unsigned)qd.x < (unsigned)nQ && (unsigned)qd.y < (unsigned)nQ && (unsigned)qd.z < (unsigned)nQ &&
-                     (unsigned)qd.w < (unsigned)nQ;
-    if (inb) {
-      float3 q0 = s4_xyz(__ldg(&Q[qd.x])), q1 = s4_xyz(__ldg(&Q[qd.y])), q2 = s4_xyz(__ldg(&Q[qd.z]));
-      rigid_fit(B, q0, q1, q2, r);
-      pass = r.ok && r.rms >= 0.f && r.rms < B.rms_threshold;  // hpp:436-439
-    }
+    pass = fit_quad(args[base], Q, nQ, quads[i], r);
   }
-  const unsigned b = __ballot_sync(0xffffffffu, pass);
-  if (b == 0u) return;
-  const int lane = threadIdx.x & 31, leader = __ffs(b) - 1;
-  uint32_t slot0 = 0;
-  if (lane == leader) slot0 = atomicAdd(nCand, (uint32_t)__popc(b));
-  slot0 = __shfl_sync(0xffffffffu, slot0, leader);
-  if (pass) {
-    const uint32_t slot = slot0 + __popc(b & ((1u << lane) - 1u));
-    candIdx[slot] = (uint32_t)i;
-    float m[12] = {r.R[0][0], r.R[0][1], r.R[0][2], r.t.x, r.R[1][0], r.R[1][1], r.R[1][2], r.t.y,
-                   r.R[2][0], r.R[2][1], r.R[2][2], r.t.z};
-    s4g_verify_record(m, ra, &outRec[slot]);
-    outRms[slot] = r.rms;
-    atomicAdd(&gateCnt[base], 1u);
-  }
+  append_candidate(pass, (uint32_t)i, r, ra, nCand, candIdx, outRec, outRms);
+  if (pass) atomicAdd(&gateCnt[base], 1u);
 }
 
 __global__ void k_bargmax(const uint32_t* __restrict__ counts, const uint32_t* __restrict__ candIdx, const uint32_t* __restrict__ nCand,
@@ -323,54 +308,18 @@ __global__ void k_bargmax(const uint32_t* __restrict__ counts, const uint32_t* _
   const uint32_t n = *nCand;
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const uint32_t t = candIdx[i], base = (uint32_t)(qkeys[t] >> kBatchSegShift);
-    const unsigned long long k = ((unsigned long long)counts[i] << 32) | (unsigned long long)(0xFFFFFFFFu - (t - quadOff[base]));
-    atomicMax(&best[base], k);
+    atomicMax(&best[base], cand_key(counts[i], t - quadOff[base]));
   }
 }
 
-// blockIdx.y = base
+// blockIdx.y = base; the key's quad index is local to the base
 __global__ void k_bfinish(const uint32_t* __restrict__ candIdx, const uint32_t* __restrict__ nCand, const VerifyCand* __restrict__ recs,
                           const float* __restrict__ rms, const unsigned long long* __restrict__ best, const BaseArgs* __restrict__ args,
                           const float4* __restrict__ Q, const int4* __restrict__ quads, const uint32_t* __restrict__ quadOff,
                           const uint32_t* __restrict__ gateCnt, int nQ, s4g_base_result* __restrict__ outs) {
   const int base = blockIdx.y;
-  s4g_tcs_result* out = &outs[base].tcs;
-  const BaseArgs B = args[base];
-  const uint32_t n = *nCand;
-  const unsigned long long key = best[base];
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    out->key = key;
-    out->n_gate_pass = gateCnt[base];
-    out->n_q = (uint32_t)nQ;
-    out->centroid1[0] = B.c1.x; out->centroid1[1] = B.c1.y; out->centroid1[2] = B.c1.z;
-    if (key == 0ull) {
-      out->best_count = 0;
-      out->best_index = -1;
-      out->best_rms = -1.f;
-      for (int i = 0; i < 16; ++i) out->best_T[i] = (i % 5 == 0) ? 1.f : 0.f;
-      out->centroid2[0] = out->centroid2[1] = out->centroid2[2] = 0.f;
-      out->best_quad[0] = out->best_quad[1] = out->best_quad[2] = out->best_quad[3] = 0;
-    }
-  }
-  if (key == 0ull) return;
-  const uint32_t widx = 0xFFFFFFFFu - (uint32_t)(key & 0xFFFFFFFFull);     // local to the base
-  const uint32_t target = quadOff[base] + widx;
-  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-    if (candIdx[i] == target) {
-      const float* T = recs[i].T;
-      out->best_count = (uint32_t)(key >> 32);
-      out->best_index = (int32_t)widx;
-      out->best_rms = rms[i];
-      for (int r = 0; r < 3; ++r)
-        for (int c = 0; c < 4; ++c) out->best_T[4 * c + r] = T[4 * r + c];
-      out->best_T[3] = out->best_T[7] = out->best_T[11] = 0.f;
-      out->best_T[15] = 1.f;
-      const int4 qd = quads[target];
-      float3 c2 = s4_div(s4_add(s4_add(s4_xyz(Q[qd.x]), s4_xyz(Q[qd.y])), s4_xyz(Q[qd.z])), 3.f);
-      out->centroid2[0] = c2.x; out->centroid2[1] = c2.y; out->centroid2[2] = c2.z;
-      out->best_quad[0] = qd.x; out->best_quad[1] = qd.y; out->best_quad[2] = qd.z; out->best_quad[3] = qd.w;
-    }
-  }
+  write_result(best[base], gateCnt[base], nQ, args[base], candIdx, *nCand, recs, rms, Q, quads, quadOff[base],
+               &outs[base].tcs);
 }
 
 }  // namespace
@@ -533,7 +482,7 @@ extern "C" int s4g_try_congruent_set_dev(s4g_ctx* ctx, const float* base_xyz, co
   }
   if (nCand > 0) {
     S4G_TRY(s4g_launch_verify(ctx, ctx->dVrec.as<VerifyCand>(), (int)nCand, ctx->dCounts.as<uint32_t>(), true, nullptr));
-    k_argmax<<<64, 256, 0, st>>>(ctx->dCounts.as<uint32_t>(), ctx->dCandIdx.as<uint32_t>(), d_nCand, d_best);
+    k_argmax<<<64, 256, 0, st>>>(ctx->dCounts.as<uint32_t>(), ctx->dCandIdx.as<uint32_t>(), d_nCand, 0u, d_best);
     ctx->launches++;
   }
   k_finish<<<64, 256, 0, st>>>(ctx->dCandIdx.as<uint32_t>(), d_nCand, ctx->dVrec.as<VerifyCand>(), ctx->dRms.as<float>(),
@@ -561,7 +510,7 @@ extern "C" int s4g_verify_best_dev(s4g_ctx* ctx, const float* d_T, int K, const 
   S4G_CUDA(cudaMemsetAsync(key, 0, sizeof(unsigned long long), st));
   if (K > 0) {
     S4G_TRY(s4g_verify_dev(ctx, d_T, K, d_counts));
-    k_argmax_n<<<64, 256, 0, st>>>(d_counts, d_index, (uint32_t)K, key);
+    k_argmax<<<64, 256, 0, st>>>(d_counts, d_index, nullptr, (uint32_t)K, key);
     ctx->launches++;
     S4G_CUDA(cudaGetLastError());
   }
