@@ -12,6 +12,7 @@
 #include "s4g_internal.cuh"
 #include <cub/cub.cuh>
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdlib>
 #include <vector>
@@ -200,8 +201,7 @@ __global__ void k_mark_bricks(GridDev g, const float4* __restrict__ P, int n, in
   if (i >= n) return;
   float4 p = P[i];
   int3 c = cell_of(g, p.x, p.y, p.z);
-  int b = ((c.z >> g.bshift) * g.tby + (c.y >> g.bshift)) * g.tbx + (c.x >> g.bshift);
-  top[b] = 1;
+  top[brick_index(g, c.x, c.y, c.z)] = 1;
 }
 
 __global__ void k_rank_bricks(int* __restrict__ top, const int* __restrict__ excl, int n) {
@@ -216,11 +216,7 @@ __global__ void k_cell_keys(GridDev g, const float4* __restrict__ P, int n, uint
   if (i >= n) return;
   float4 p = P[i];
   int3 c = cell_of(g, p.x, p.y, p.z);
-  int bs = g.bshift, m = (1 << bs) - 1;
-  int b = ((c.z >> bs) * g.tby + (c.y >> bs)) * g.tbx + (c.x >> bs);
-  uint32_t rank = (uint32_t)g.top[b];
-  uint32_t local = (uint32_t)((((c.z & m) << bs) | (c.y & m)) << bs) | (uint32_t)(c.x & m);
-  uint32_t key = (rank << (3 * bs)) | local;
+  uint32_t key = cell_slot(g, g.top[brick_index(g, c.x, c.y, c.z)], c.x, c.y, c.z);
   keys[i] = key;
   vals[i] = (uint32_t)i;
   atomicAdd(&cellCount[key], 1u);
@@ -243,17 +239,16 @@ __global__ void k_mark_vocc(GridDev g, const float4* __restrict__ P, int n, uint
   if (i >= n) return;
   float4 p = P[i];
   int3 c = cell_of(g, p.x, p.y, p.z);
-  const int bs = g.bshift, m = (1 << bs) - 1;
 #pragma unroll
   for (int d = 0; d < 8; ++d) {
     const int dx = d & 1, dy = (d >> 1) & 1, dz = d >> 2;
     const int ox = c.x - dx, oy = c.y - dy, oz = c.z - dz;
     if (ox < 0 || oy < 0 || oz < 0) { atomicAdd(err, 1u); continue; }
-    const int rank = g.vtop[((oz >> bs) * g.tby + (oy >> bs)) * g.tbx + (ox >> bs)];
+    const int rank = g.vtop[brick_index(g, ox, oy, oz)];
     if (rank < 0) { atomicAdd(err, 1u); continue; }              // cannot happen: k_mark_vbricks marks every origin's brick
-    const uint32_t cell = ((uint32_t)rank << (3 * bs)) | (uint32_t)((((oz & m) << bs) | (oy & m)) << bs) | (uint32_t)(ox & m);
-    const uint32_t bit = 1u << ((cell & 7u) * 4u + (uint32_t)(dz * 2 + dy));
-    if (!(vocc[cell >> 3] & bit)) atomicOr(&vocc[cell >> 3], bit);
+    const uint32_t cell = cell_slot(g, rank, ox, oy, oz);
+    const uint32_t bit = 1u << (vocc_shift(cell) + (uint32_t)(dz * 2 + dy));
+    if (!(vocc[vocc_word(cell)] & bit)) atomicOr(&vocc[vocc_word(cell)], bit);
   }
 }
 
@@ -290,25 +285,23 @@ __global__ void k_mark_vbricks(GridDev g, const float4* __restrict__ P, int n, f
   for (int d = 0; d < 8; ++d) {
     int3 c = cell_of(g, p.x + ((d & 1) ? reach : -reach), p.y + ((d & 2) ? reach : -reach),
                      p.z + ((d & 4) ? reach : -reach));
-    vtop[((c.z >> g.bshift) * g.tby + (c.y >> g.bshift)) * g.tbx + (c.x >> g.bshift)] = 1;
+    vtop[brick_index(g, c.x, c.y, c.z)] = 1;
   }
   // ... and the origin cells c - (dx, dy, dz) of the 2x2x2 blocks that contain the point's cell (GridDev::vocc lives there)
   const int3 c = cell_of(g, p.x, p.y, p.z);
 #pragma unroll
   for (int d = 0; d < 8; ++d) {
     const int ox = max(c.x - (d & 1), 0), oy = max(c.y - ((d >> 1) & 1), 0), oz = max(c.z - (d >> 2), 0);
-    vtop[((oz >> g.bshift) * g.tby + (oy >> g.bshift)) * g.tbx + (ox >> g.bshift)] = 1;
+    vtop[brick_index(g, ox, oy, oz)] = 1;
   }
 }
 
-// One warp per P point: classify the (2R+1)^3 voxels around it.  Voxel k spans [ox + k v, ox + (k+1) v) per axis with
-// v = 1 / inv_v (the lattice verify.cu's floor(V q) addresses); the box is inflated by `slack` (position uncertainty of
-// the query's voxel) and the radius by +-md (rounding of the fp32 decision d^2 <= delta^2), so that
-//   MAYBE clear   =>  no location of the voxel is within delta of this point  (for every point: no inlier possible)
-//   CERTAIN set   =>  every location of the voxel is within delta of this point (inlier, whatever the exact position)
-// Arithmetic in double: the classification has to be conservative, not bit-compatible with anything.
-__global__ void k_mark_voxels(GridDev g, const float4* __restrict__ P, int n, int R, double delta, double slack,
-                              double md, uint32_t* __restrict__ vox, unsigned int* __restrict__ err) {
+// The delta-field builders: one warp per P point visits each of the (2R+1)^3 voxels around it inside the lattice; voxel k
+// spans [ox + k v, ox + (k+1) v) per axis, v = 1 / inv_v.  Double: conservative, not bit-compatible with anything.
+struct FieldPoint { double px, py, pz, ox, oy, oz, v, r_maybe, r_cert; };
+template <class Visit>
+__device__ __forceinline__ void for_voxels_near(const GridDev& g, const float4* __restrict__ P, int n, int R, double delta,
+                                                double md, Visit visit) {
   const long long gw = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (gw >= n) return;
@@ -318,100 +311,116 @@ __global__ void k_mark_voxels(GridDev g, const float4* __restrict__ P, int n, in
   const long long kx = (long long)floor((px - ox) / v), ky = (long long)floor((py - oy) / v),
                   kz = (long long)floor((pz - oz) / v);
   const int side = 2 * R + 1, total = side * side * side;
-  const double r_maybe = (delta + md) * (delta + md);
-  const double r_cert = delta > md ? (delta - md) * (delta - md) : -1.0;
-  const int bs = g.bshift, m = (1 << bs) - 1;
+  const FieldPoint f{px, py, pz, ox, oy, oz, v, (delta + md) * (delta + md), delta > md ? (delta - md) * (delta - md) : -1.0};
   for (int o = lane; o < total; o += 32) {
     const int dz = o / (side * side) - R, dy = (o / side) % side - R, dx = o % side - R;
     const long long X = kx + dx, Y = ky + dy, Z = kz + dz;
     if (X < 0 || Y < 0 || Z < 0 || X >= 4ll * g.nx || Y >= 4ll * g.ny || Z >= 4ll * g.nz) continue;
-    const double lx = ox + (double)X * v - slack, hx = ox + (double)(X + 1) * v + slack;
-    const double ly = oy + (double)Y * v - slack, hy = oy + (double)(Y + 1) * v + slack;
-    const double lz = oz + (double)Z * v - slack, hz = oz + (double)(Z + 1) * v + slack;
-    const double nx_ = fmax(0.0, fmax(lx - px, px - hx)), ny_ = fmax(0.0, fmax(ly - py, py - hy)),
-                 nz_ = fmax(0.0, fmax(lz - pz, pz - hz));
-    const double fx = fmax(px - lx, hx - px), fy = fmax(py - ly, hy - py), fz = fmax(pz - lz, hz - pz);
-    const double dmin2 = nx_ * nx_ + ny_ * ny_ + nz_ * nz_, dmax2 = fx * fx + fy * fy + fz * fz;
-    if (!(dmin2 <= r_maybe)) continue;
-    const int cx = (int)(X >> 2), cy = (int)(Y >> 2), cz = (int)(Z >> 2);
-    const int rank = g.vtop[((cz >> bs) * g.tby + (cy >> bs)) * g.tbx + (cx >> bs)];
-    if (rank < 0) { atomicAdd(err, 1u); continue; }   // cannot happen (k_mark_vbricks is a superset); checked by the host
-    const uint32_t local = (uint32_t)((((cz & m) << bs) | (cy & m)) << bs) | (uint32_t)(cx & m);
-    const size_t word = ((((size_t)rank << (3 * bs)) | local) << 2) | (size_t)(Z & 3);
-    const uint32_t sh = 2u * (uint32_t)(((Y & 3) << 2) | (X & 3));
-    const uint32_t bits = (dmax2 <= r_cert ? 3u : 1u) << sh;
-    if ((vox[word] & bits) != bits) atomicOr(&vox[word], bits);
+    visit((int)X, (int)Y, (int)Z, f);
   }
 }
+// squared distances from the point of f to the nearest (x) and the farthest (y) location of the box [lo, hi]
+__device__ __forceinline__ double2 box_dist2(const FieldPoint& f, double lx, double ly, double lz, double hx, double hy,
+                                             double hz) {
+  const double nx_ = fmax(0.0, fmax(lx - f.px, f.px - hx)), ny_ = fmax(0.0, fmax(ly - f.py, f.py - hy)),
+               nz_ = fmax(0.0, fmax(lz - f.pz, f.pz - hz));
+  const double fx = fmax(f.px - lx, hx - f.px), fy = fmax(f.py - ly, hy - f.py), fz = fmax(f.pz - lz, hz - f.pz);
+  return make_double2(nx_ * nx_ + ny_ * ny_ + nz_ * nz_, fx * fx + fy * fy + fz * fz);
+}
 
-// boundary voxels (MAYBE, not CERTAIN) of a 32-bit slab word of the delta-field: bit 2k set <=> voxel k is one
-__device__ __forceinline__ uint32_t boundary_bits(uint32_t w) { return w & ~(w >> 1) & 0x55555555u; }
+// Classify the voxels around every P point.  The box is inflated by `slack` (position uncertainty of the query's voxel)
+// and the radius by +-md (rounding of the fp32 decision d^2 <= delta^2), so that
+//   MAYBE clear   =>  no location of the voxel is within delta of this point  (for every point: no inlier possible)
+//   CERTAIN set   =>  every location of the voxel is within delta of this point (inlier, whatever the exact position)
+__global__ void k_mark_voxels(GridDev g, const float4* __restrict__ P, int n, int R, double delta, double slack,
+                              double md, uint32_t* __restrict__ vox, unsigned int* __restrict__ err) {
+  for_voxels_near(g, P, n, R, delta, md, [&](int X, int Y, int Z, const FieldPoint& f) {
+    const double2 d = box_dist2(f, f.ox + (double)X * f.v - slack, f.oy + (double)Y * f.v - slack, f.oz + (double)Z * f.v - slack,
+                                f.ox + (double)(X + 1) * f.v + slack, f.oy + (double)(Y + 1) * f.v + slack,
+                                f.oz + (double)(Z + 1) * f.v + slack);
+    if (!(d.x <= f.r_maybe)) return;
+    const int rank = g.vtop[brick_index<0, 2>(g, X, Y, Z)];
+    if (rank < 0) { atomicAdd(err, 1u); return; }   // cannot happen (k_mark_vbricks is a superset); checked by the host
+    const uint32_t word = vox_word(vox_cell(g, rank, X, Y, Z), Z);
+    const uint32_t bits = (d.y <= f.r_cert ? 3u : 1u) << vox_shift(X, Y);
+    if ((vox[word] & bits) != bits) atomicOr(&vox[word], bits);
+  });
+}
 
 // per cell of the v-bricks: number of boundary voxels (-> exclusive scan = GridDev::vbase)
 __global__ void k_count_boundary(const uint32_t* __restrict__ vox, long long nCells, uint32_t* __restrict__ counts) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= nCells) return;
-  const uint4 w = reinterpret_cast<const uint4*>(vox)[i];
+  const uint4 w = vox_cells(vox)[i];
   counts[i] = (uint32_t)(__popc(boundary_bits(w.x)) + __popc(boundary_bits(w.y)) + __popc(boundary_bits(w.z)) +
                          __popc(boundary_bits(w.w)));
 }
 
 // Second level of the delta-field: for every boundary voxel within reach of a point, classify its 2x2x2 sub-voxels
-// against that point exactly like k_mark_voxels classifies voxels (same margins).  One warp per P point.
+// against that point exactly like k_mark_voxels classifies voxels (same margins).
 __global__ void k_mark_subvoxels(GridDev g, const float4* __restrict__ P, int n, int R, double delta, double slack,
                                  double md, uint32_t* __restrict__ fine32) {
-  const long long gw = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (gw >= n) return;
-  const float4 pf = P[gw];
-  const double v = 1.0 / (double)g.inv_v, hv = 0.5 * v;
-  const double px = pf.x, py = pf.y, pz = pf.z, ox = g.ox, oy = g.oy, oz = g.oz;
-  const long long kx = (long long)floor((px - ox) / v), ky = (long long)floor((py - oy) / v),
-                  kz = (long long)floor((pz - oz) / v);
-  const int side = 2 * R + 1, total = side * side * side;
-  const double r_maybe = (delta + md) * (delta + md);
-  const double r_cert = delta > md ? (delta - md) * (delta - md) : -1.0;
-  const int bs = g.bshift, m = (1 << bs) - 1;
-  for (int o = lane; o < total; o += 32) {
-    const int dz = o / (side * side) - R, dy = (o / side) % side - R, dx = o % side - R;
-    const long long X = kx + dx, Y = ky + dy, Z = kz + dz;
-    if (X < 0 || Y < 0 || Z < 0 || X >= 4ll * g.nx || Y >= 4ll * g.ny || Z >= 4ll * g.nz) continue;
-    const double lx = ox + (double)X * v, ly = oy + (double)Y * v, lz = oz + (double)Z * v;   // voxel's low corner
-    {
-      const double nx_ = fmax(0.0, fmax(lx - slack - px, px - (lx + v + slack))), ny_ = fmax(0.0, fmax(ly - slack - py, py - (ly + v + slack))),
-                   nz_ = fmax(0.0, fmax(lz - slack - pz, pz - (lz + v + slack)));
-      if (!(nx_ * nx_ + ny_ * ny_ + nz_ * nz_ <= r_maybe)) continue;          // no child can be MAYBE for this point
-    }
-    const int cx = (int)(X >> 2), cy = (int)(Y >> 2), cz = (int)(Z >> 2);
-    const int rank = g.vtop[((cz >> bs) * g.tby + (cy >> bs)) * g.tbx + (cx >> bs)];
-    if (rank < 0) continue;
-    const uint32_t cell = ((uint32_t)rank << (3 * bs)) | (uint32_t)((((cz & m) << bs) | (cy & m)) << bs) | (uint32_t)(cx & m);
-    const uint4 cw = reinterpret_cast<const uint4*>(g.vox)[cell];
-    const uint32_t ws[4] = {cw.x, cw.y, cw.z, cw.w};
-    const int vz = (int)(Z & 3);
-    const uint32_t sh = 2u * (uint32_t)(((Y & 3) << 2) | (X & 3));
-    if (((boundary_bits(ws[vz]) >> sh) & 1u) == 0u) continue;                 // voxel decided at the first level
-    uint32_t slot = g.vbase[cell] + (uint32_t)__popc(boundary_bits(ws[vz]) & ((1u << sh) - 1u));
-    for (int k = 0; k < vz; ++k) slot += (uint32_t)__popc(boundary_bits(ws[k]));
+  for_voxels_near(g, P, n, R, delta, md, [&](int X, int Y, int Z, const FieldPoint& f) {
+    const double v = f.v, hv = 0.5 * v;
+    const double lx = f.ox + (double)X * v, ly = f.oy + (double)Y * v, lz = f.oz + (double)Z * v;   // voxel's low corner
+    if (!(box_dist2(f, lx - slack, ly - slack, lz - slack, lx + v + slack, ly + v + slack, lz + v + slack).x <= f.r_maybe))
+      return;                                                                   // no child can be MAYBE for this point
+    const int rank = g.vtop[brick_index<0, 2>(g, X, Y, Z)];
+    if (rank < 0) return;
+    const uint32_t cell = vox_cell(g, rank, X, Y, Z);
+    const uint4 cw = vox_cells(g.vox)[cell];
+    const uint32_t ws[4] = {cw.x, cw.y, cw.z, cw.w}, w = ws[Z & 3];
+    const uint32_t sh = vox_shift(X, Y);
+    if (((boundary_bits(w) >> sh) & 1u) == 0u) return;                        // voxel decided at the first level
+    const uint32_t slot = boundary_slot(g.vbase[cell], cw, w, Z & 3, sh);
     uint32_t bits = 0u;
 #pragma unroll
     for (int ch = 0; ch < 8; ++ch) {
       const double ax = lx + ((ch & 1) ? hv : 0.0) - slack, bx = ax + hv + 2.0 * slack;
       const double ay = ly + ((ch & 2) ? hv : 0.0) - slack, by = ay + hv + 2.0 * slack;
       const double az = lz + ((ch & 4) ? hv : 0.0) - slack, bz = az + hv + 2.0 * slack;
-      const double mx_ = fmax(0.0, fmax(ax - px, px - bx)), my_ = fmax(0.0, fmax(ay - py, py - by)), mz_ = fmax(0.0, fmax(az - pz, pz - bz));
-      const double fx = fmax(px - ax, bx - px), fy = fmax(py - ay, by - py), fz = fmax(pz - az, bz - pz);
-      if (mx_ * mx_ + my_ * my_ + mz_ * mz_ <= r_maybe) bits |= 1u << ch;
-      if (fx * fx + fy * fy + fz * fz <= r_cert) bits |= 0x101u << ch;        // CERTAIN implies MAYBE
+      const double2 d = box_dist2(f, ax, ay, az, bx, by, bz);
+      if (d.x <= f.r_maybe) bits |= fine_maybe(ch);
+      if (d.y <= f.r_cert) bits |= fine_certain(ch);
     }
     if (bits) {
-      const uint32_t word = slot >> 1, s16 = (slot & 1u) * 16u;
+      const uint32_t word = fine_word(slot), s16 = fine_half(slot);
       if (((fine32[word] >> s16) & bits) != bits) atomicOr(&fine32[word], bits << s16);
     }
-  }
+  });
 }
 
 static inline int nblk(long long n, int t) { return (int)((n + t - 1) / t); }
+
+// brick flags (1 = marked) -> ranks (exclusive prefix, -1 where unmarked), count = marked bricks; count >= limit fails first
+static int rank_flags(s4g_ctx* ctx, int* flags, long long ntop, long long limit, const char* too_many, long long& count) {
+  cudaStream_t st = ctx->stream;
+  size_t cub_bytes = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, flags, ctx->dScratchB.as<int>(), (int)ntop, st);
+  S4G_TRY(s4g_reserve(ctx, ctx->dCub, cub_bytes));
+  cub::DeviceScan::ExclusiveSum(ctx->dCub.p, cub_bytes, flags, ctx->dScratchB.as<int>(), (int)ntop, st);
+  int last_flag = 0, last_excl = 0;
+  S4G_CUDA(cudaMemcpyAsync(&last_flag, flags + (ntop - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
+  S4G_CUDA(cudaMemcpyAsync(&last_excl, ctx->dScratchB.as<int>() + (ntop - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
+  S4G_CUDA(cudaStreamSynchronize(st));
+  count = (long long)last_flag + last_excl;
+  if (count >= limit) { ctx->err = too_many; return S4G_ERR_NOMEM; }
+  k_rank_bricks<<<nblk(ntop, 256), 256, 0, st>>>(flags, ctx->dScratchB.as<int>(), (int)ntop);
+  return S4G_OK;
+}
+
+// zero the error word dMisc[0], enqueue launch(word), then fail with `msg` if a thread counted an error in it
+template <class Launch>
+static int launch_checked(s4g_ctx* ctx, const char* msg, Launch launch) {
+  S4G_CUDA(cudaMemsetAsync(ctx->dMisc.p, 0, 4, ctx->stream));
+  launch(ctx->dMisc.as<unsigned int>());
+  S4G_CUDA(cudaGetLastError());
+  unsigned int err = 0;
+  S4G_CUDA(cudaMemcpyAsync(&err, ctx->dMisc.p, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  S4G_CUDA(cudaStreamSynchronize(ctx->stream));
+  if (err) { ctx->err = msg; return S4G_ERR_CUDA; }
+  return S4G_OK;
+}
 
 extern "C" int s4g_set_cloud_p(s4g_ctx* ctx, const float* xyz, int n, float delta) {
   if (!ctx) return S4G_ERR_ARG;
@@ -473,21 +482,10 @@ extern "C" int s4g_set_cloud_p(s4g_ctx* ctx, const float* xyz, int n, float delt
   S4G_CUDA(cudaMemsetAsync(ctx->dTop.p, 0, (size_t)ntop * sizeof(int), st));
   g.top = ctx->dTop.as<int>();
   k_mark_bricks<<<nblk(n, 256), 256, 0, st>>>(g, ctx->dP.as<float4>(), n, ctx->dTop.as<int>());
-  size_t cub_bytes = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, ctx->dTop.as<int>(), ctx->dScratchB.as<int>(), (int)ntop, st);
-  S4G_TRY(s4g_reserve(ctx, ctx->dCub, cub_bytes));
-  cub::DeviceScan::ExclusiveSum(ctx->dCub.p, cub_bytes, ctx->dTop.as<int>(), ctx->dScratchB.as<int>(), (int)ntop, st);
-  int last_flag = 0, last_excl = 0;
-  S4G_CUDA(cudaMemcpyAsync(&last_flag, ctx->dTop.as<int>() + (ntop - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
-  S4G_CUDA(cudaMemcpyAsync(&last_excl, ctx->dScratchB.as<int>() + (ntop - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
-  S4G_CUDA(cudaStreamSynchronize(st));
-  long long nBricks = (long long)last_flag + last_excl;
+  long long nBricks = 0;
+  S4G_TRY(rank_flags(ctx, ctx->dTop.as<int>(), ntop, 1ll << (31 - 3 * bs),   // i.e. nBricks << 3*bs cells >= 2^31
+                     "s4g_set_cloud_p: grid too large (cells >= 2^31); delta too small for this cloud", nBricks));
   long long nCells = nBricks << (3 * bs);
-  if (nCells >= (1ll << 31)) {
-    ctx->err = "s4g_set_cloud_p: grid too large (cells >= 2^31); delta too small for this cloud";
-    return S4G_ERR_NOMEM;
-  }
-  k_rank_bricks<<<nblk(ntop, 256), 256, 0, st>>>(ctx->dTop.as<int>(), ctx->dScratchB.as<int>(), (int)ntop);
 
   S4G_TRY(s4g_reserve(ctx, ctx->dCellStart, (size_t)(nCells + 1) * sizeof(uint32_t)));
   S4G_TRY(s4g_reserve(ctx, ctx->dScratchC, (size_t)(nCells + 1) * sizeof(uint32_t)));  // counts
@@ -501,7 +499,7 @@ extern "C" int s4g_set_cloud_p(s4g_ctx* ctx, const float* xyz, int n, float delt
                                             ctx->dScratchC.as<uint32_t>());
   int key_bits = 1;
   while ((1ll << key_bits) < nCells && key_bits < 32) ++key_bits;
-  cub_bytes = 0;
+  size_t cub_bytes = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, keys_in, keys_out, vals_in, vals_out, n, 0, key_bits, st);
   size_t scan_bytes = 0;
   cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, ctx->dScratchC.as<uint32_t>(),
@@ -561,16 +559,8 @@ extern "C" int s4g_set_cloud_p(s4g_ctx* ctx, const float* xyz, int n, float delt
     S4G_CUDA(cudaMemsetAsync(ctx->dVtop.p, 0, (size_t)ntop * sizeof(int), st));
     k_mark_vbricks<<<nblk(n, 256), 256, 0, st>>>(g, ctx->dP.as<float4>(), n, (float)(reach * 1.05 + 1e-3 * h),
                                                  ctx->dVtop.as<int>());
-    cub_bytes = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, ctx->dVtop.as<int>(), ctx->dScratchB.as<int>(), (int)ntop, st);
-    S4G_TRY(s4g_reserve(ctx, ctx->dCub, cub_bytes));
-    cub::DeviceScan::ExclusiveSum(ctx->dCub.p, cub_bytes, ctx->dVtop.as<int>(), ctx->dScratchB.as<int>(), (int)ntop, st);
-    int vlast_flag = 0, vlast_excl = 0;
-    S4G_CUDA(cudaMemcpyAsync(&vlast_flag, ctx->dVtop.as<int>() + (ntop - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
-    S4G_CUDA(cudaMemcpyAsync(&vlast_excl, ctx->dScratchB.as<int>() + (ntop - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
-    S4G_CUDA(cudaStreamSynchronize(st));
-    const long long nVB = (long long)vlast_flag + vlast_excl;
-    k_rank_bricks<<<nblk(ntop, 256), 256, 0, st>>>(ctx->dVtop.as<int>(), ctx->dScratchB.as<int>(), (int)ntop);
+    long long nVB = 0;
+    S4G_TRY(rank_flags(ctx, ctx->dVtop.as<int>(), ntop, LLONG_MAX, nullptr, nVB));
     const size_t vwords = ((size_t)nVB << (3 * bs)) * 4;
     if (vwords >= (size_t(1) << 32)) {
       ctx->err = "s4g_set_cloud_p: delta-field too large (>= 16 GiB); delta too small for this cloud";
@@ -579,31 +569,23 @@ extern "C" int s4g_set_cloud_p(s4g_ctx* ctx, const float* xyz, int n, float delt
     S4G_TRY(s4g_reserve(ctx, ctx->dVox, std::max<size_t>(vwords, 4) * sizeof(uint32_t)));
     S4G_TRY(s4g_reserve(ctx, ctx->dMisc, 256));
     S4G_CUDA(cudaMemsetAsync(ctx->dVox.p, 0, std::max<size_t>(vwords, 4) * sizeof(uint32_t), st));
-    S4G_CUDA(cudaMemsetAsync(ctx->dMisc.p, 0, 4, st));
     g.vtop = ctx->dVtop.as<int>();
     g.vox = ctx->dVox.as<uint32_t>();
-    k_mark_voxels<<<nblk((long long)n * 32, 256), 256, 0, st>>>(g, ctx->dP.as<float4>(), n, R, (double)delta, slack, md,
-                                                                ctx->dVox.as<uint32_t>(), ctx->dMisc.as<unsigned int>());
     ctx->launches += 5;
-    S4G_CUDA(cudaGetLastError());
-    unsigned int verr = 0;
-    S4G_CUDA(cudaMemcpyAsync(&verr, ctx->dMisc.p, 4, cudaMemcpyDeviceToHost, st));
-    S4G_CUDA(cudaStreamSynchronize(st));
-    if (verr) { ctx->err = "s4g_set_cloud_p: internal error (delta-field voxel outside its v-bricks)"; return S4G_ERR_CUDA; }
+    S4G_TRY(launch_checked(ctx, "s4g_set_cloud_p: internal error (delta-field voxel outside its v-bricks)", [&](unsigned int* err) {
+      k_mark_voxels<<<nblk((long long)n * 32, 256), 256, 0, st>>>(g, ctx->dP.as<float4>(), n, R, (double)delta, slack, md,
+                                                                  ctx->dVox.as<uint32_t>(), err);
+    }));
     ctx->nVBricks = nVB;
     {
       // occupancy nibbles of the blocks the exact test probes, per origin cell of the v-bricks
       const size_t owords = (size_t)((nVB << (3 * bs)) + 7) / 8 + 1;
       S4G_TRY(s4g_reserve(ctx, ctx->dVocc, owords * sizeof(uint32_t)));
       S4G_CUDA(cudaMemsetAsync(ctx->dVocc.p, 0, owords * sizeof(uint32_t), st));
-      S4G_CUDA(cudaMemsetAsync(ctx->dMisc.p, 0, 4, st));
-      k_mark_vocc<<<nblk(n, 256), 256, 0, st>>>(g, ctx->dP.as<float4>(), n, ctx->dVocc.as<uint32_t>(), ctx->dMisc.as<unsigned int>());
       ctx->launches++;
-      S4G_CUDA(cudaGetLastError());
-      unsigned int oerr = 0;
-      S4G_CUDA(cudaMemcpyAsync(&oerr, ctx->dMisc.p, 4, cudaMemcpyDeviceToHost, st));
-      S4G_CUDA(cudaStreamSynchronize(st));
-      if (oerr) { ctx->err = "s4g_set_cloud_p: internal error (block origin outside the v-bricks)"; return S4G_ERR_CUDA; }
+      S4G_TRY(launch_checked(ctx, "s4g_set_cloud_p: internal error (block origin outside the v-bricks)", [&](unsigned int* err) {
+        k_mark_vocc<<<nblk(n, 256), 256, 0, st>>>(g, ctx->dP.as<float4>(), n, ctx->dVocc.as<uint32_t>(), err);
+      }));
       g.vocc = ctx->dVocc.as<uint32_t>();
     }
     // second level: sub-voxel bits of the boundary voxels
@@ -674,11 +656,13 @@ extern "C" int s4g_get_grid_stats(s4g_ctx* ctx, double* out6) {
   return S4G_OK;
 }
 
+// Every term is a whole number of bytes (vocc: half a byte per cell) far below 2^53, so the sum is exact in any order.
 double s4g_grid_bytes(const s4g_ctx* ctx) {
-  const long long ntop = (long long)ctx->grid.tbx * ctx->grid.tby * ctx->grid.tbz;
-  return (double)ctx->nP * 16.0 + (double)(ctx->nCells + 1) * 4.0 + (double)ntop * 4.0 +
-         (double)ntop * 4.0 + (double)(ctx->nVBricks << (3 * ctx->grid.bshift)) * 0.5 +
-         (double)(ctx->nVBricks << (3 * ctx->grid.bshift)) * 20.0 + (double)ctx->nVBoundary * 2.0;
+  const double ntop = (double)ctx->grid.tbx * ctx->grid.tby * ctx->grid.tbz;
+  const double vcells = (double)(ctx->nVBricks << (3 * ctx->grid.bshift));
+  const double pts = 16.0 * ctx->nP, cellStart = 4.0 * (ctx->nCells + 1), top = 4.0 * ntop, vtop = 4.0 * ntop;
+  const double vocc = 0.5 * vcells, vox = 16.0 * vcells, vbase = 4.0 * vcells, vfine = 2.0 * ctx->nVBoundary;
+  return pts + cellStart + top + vtop + vocc + vox + vbase + vfine;
 }
 
 // =============================================================================================
@@ -703,14 +687,7 @@ __global__ void k_pack_q(const float* __restrict__ xyz, const float* __restrict_
   uint32_t ux = min(1023u, (uint32_t)max(0.f, (x - bx) * mscale));
   uint32_t uy = min(1023u, (uint32_t)max(0.f, (y - by) * mscale));
   uint32_t uz = min(1023u, (uint32_t)max(0.f, (z - bz) * mscale));
-  auto spread = [](uint32_t v) {
-    v = (v | (v << 16)) & 0x030000FFu;
-    v = (v | (v << 8)) & 0x0300F00Fu;
-    v = (v | (v << 4)) & 0x030C30C3u;
-    v = (v | (v << 2)) & 0x09249249u;
-    return v;
-  };
-  mkeys[i] = spread(ux) | (spread(uy) << 1) | (spread(uz) << 2);
+  mkeys[i] = morton_spread10(ux) | (morton_spread10(uy) << 1) | (morton_spread10(uz) << 2);
   mvals[i] = (uint32_t)i;
 }
 
@@ -729,15 +706,7 @@ __global__ void k_tile_spheres(const float4* __restrict__ qm, int n, int nTiles,
       hi.x = fmaxf(hi.x, a.x); hi.y = fmaxf(hi.y, a.y); hi.z = fmaxf(hi.z, a.z);
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    lo.x = fminf(lo.x, __shfl_xor_sync(0xffffffffu, lo.x, o));
-    lo.y = fminf(lo.y, __shfl_xor_sync(0xffffffffu, lo.y, o));
-    lo.z = fminf(lo.z, __shfl_xor_sync(0xffffffffu, lo.z, o));
-    hi.x = fmaxf(hi.x, __shfl_xor_sync(0xffffffffu, hi.x, o));
-    hi.y = fmaxf(hi.y, __shfl_xor_sync(0xffffffffu, hi.y, o));
-    hi.z = fmaxf(hi.z, __shfl_xor_sync(0xffffffffu, hi.z, o));
-  }
+  warp_aabb(lo, hi);
   float3 c = make_float3(0.5f * (lo.x + hi.x), 0.5f * (lo.y + hi.y), 0.5f * (lo.z + hi.z));
   float r2 = 0.f;
   for (int k = lane; k < tile; k += 32) {

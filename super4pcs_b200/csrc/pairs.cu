@@ -418,15 +418,7 @@ __global__ void k_group_boxes(const float4* __restrict__ lo_in, const float4* __
       hi.x = fmaxf(hi.x, b.x); hi.y = fmaxf(hi.y, b.y); hi.z = fmaxf(hi.z, b.z);
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    lo.x = fminf(lo.x, __shfl_xor_sync(0xffffffffu, lo.x, o));
-    lo.y = fminf(lo.y, __shfl_xor_sync(0xffffffffu, lo.y, o));
-    lo.z = fminf(lo.z, __shfl_xor_sync(0xffffffffu, lo.z, o));
-    hi.x = fmaxf(hi.x, __shfl_xor_sync(0xffffffffu, hi.x, o));
-    hi.y = fmaxf(hi.y, __shfl_xor_sync(0xffffffffu, hi.y, o));
-    hi.z = fmaxf(hi.z, __shfl_xor_sync(0xffffffffu, hi.z, o));
-  }
+  warp_aabb(lo, hi);
   if (lane == 0) {
     lo_out[g] = make_float4(lo.x, lo.y, lo.z, 0.f);
     hi_out[g] = make_float4(hi.x, hi.y, hi.z, 0.f);

@@ -35,14 +35,15 @@ struct DevBuf {
 // (edge 2^bshift cells) holds the rank of each occupied brick; occupied bricks own a dense
 // block of cellStart entries; P is sorted by (brick rank, local cell) so every cell -- and
 // every x-adjacent cell pair inside a brick -- is one contiguous run of float4 points.
+// The address arithmetic of every table is defined once, by the helpers below the struct.
 struct GridDev {
   float ox, oy, oz;     // world coordinate of cell (0,0,0)'s low corner
   float inv_h;          // 1 / cell edge
   int nx, ny, nz;       // extent in cells
   int bshift;           // log2(brick edge in cells)
   int tbx, tby, tbz;    // extent in bricks
-  const int* top;       // [tbx*tby*tbz] brick rank or -1
-  const uint32_t* cellStart;  // [(nBricks << 3*bshift) + 1]
+  const int* top;       // [tbx*tby*tbz] brick rank or -1 (brick_index)
+  const uint32_t* cellStart;  // [(nBricks << 3*bshift) + 1] (cell_slot)
   const float4* pts;    // sorted points, w = original index (bit pattern)
   const uint32_t* csat; // summed-area table of the coarse occupancy ((2^cshift)^3-cell blocks):
                         // csat[(Z*(cny+1)+Y)*(cnx+1)+X] = #occupied blocks with x<X, y<Y, z<Z; or nullptr
@@ -51,21 +52,95 @@ struct GridDev {
   // (the bricks of `top`'s lattice that hold at least one voxel within delta of a P point): bit 0 = MAYBE (some P
   // point may lie within delta of some location of the voxel), bit 1 = CERTAIN (one P point lies within delta of
   // EVERY location of the voxel).  Neither bit: no P point within delta of any location of the voxel.
-  const int* vtop;      // [tbx*tby*tbz] v-brick rank or -1
-  const uint32_t* vox;  // [nVBricks << (3*bshift + 2)] words: (rank << (3*bshift) | local cell) * 4 + (vz & 3); bits 2*((vy&3)*4 + (vx&3))
-  // second level, for the BOUNDARY voxels (MAYBE but not CERTAIN) only: the same two bits for each of the voxel's 2x2x2
-  // sub-voxels (edge h/8 ~ delta/4).  vbase[cell] = slot of the cell's first boundary voxel (cells in v-brick order, voxels
-  // in bit order of the cell's 4 words); vfine[slot] = MAYBE bits of the 8 children (bits 0-7, child = sx | sy << 1 | sz << 2)
-  // | CERTAIN bits (bits 8-15).
-  // occupancy of the 2x2x2-cell blocks the exact test probes: 4 bits per block ORIGIN cell (which of the block's four x-rows
-  // hold points), stored for the cells of the v-bricks only (every origin of a non-empty block lies in one): nibble
-  // (rank << 3*bshift | local cell) of vocc
+  const int* vtop;      // [tbx*tby*tbz] v-brick rank or -1 (brick_index<0, 2>)
+  const uint32_t* vox;  // [nVBricks << (3*bshift + 2)] words (vox_cell, vox_word, vox_shift)
+  // vbase, vfine: for the BOUNDARY voxels (MAYBE, not CERTAIN) the same bits of their 2x2x2 sub-voxels (boundary_slot, fine_*);
+  // vocc: which x-rows of each 2x2x2-cell block the exact test probes hold points, per v-brick cell (vocc_word, vocc_shift)
   const uint32_t* vocc;
   const uint32_t* vbase;
   const uint16_t* vfine;
   float inv_v;          // 4 * inv_h (voxels per world unit)
   float vslack;         // world-unit uncertainty of a query's voxel position the field was built to tolerate
 };
+
+// ---- table layouts of GridDev: written by s4g_set_cloud_p (context.cu), read by k_verify (verify.cu).  kBS > 0: the
+// brick shift known at compile time (2 = the common 4x4x4-cell bricks), 0: read from the grid.  bs = log2(brick edge),
+// m = brick edge - 1; kSub = 2 addresses the bricks by voxel of the delta-field (4 per cell edge) instead of by cell.
+struct BrickShape { int bs, m; };
+template <int kBS = 0>
+__device__ __forceinline__ BrickShape brick_shape(const GridDev& g, int sub = 0) {
+  const int bs = kBS > 0 ? kBS : g.bshift; return BrickShape{bs + sub, (1 << bs) - 1};
+}
+// top / vtop: index of the brick that holds cell (x, y, z) = the first brick of its row (y, z) + x >> bs
+__device__ __forceinline__ int brick_row(const GridDev& g, BrickShape b, int y, int z) { return ((z >> b.bs) * g.tby + (y >> b.bs)) * g.tbx; }
+__device__ __forceinline__ int brick_in_row(BrickShape b, int row, int x) { return row + (x >> b.bs); }
+template <int kBS = 0, int kSub = 0>
+__device__ __forceinline__ int brick_index(const GridDev& g, int x, int y, int z) {
+  const BrickShape b = brick_shape<kBS>(g, kSub);
+  return brick_in_row(b, brick_row(g, b, y, z), x);
+}
+// cellStart, vocc, vbase (and vox, 4 words per slot): slot of cell (x, y, z) in the brick of rank `rank` = rank << 3*bs |
+// local cell (z, y, x bits), so that a brick's cells, and an x-row's cells, are consecutive; cell_row = the row's bits
+__device__ __forceinline__ uint32_t cell_row(BrickShape b, int y, int z) { return (uint32_t)((((z & b.m) << b.bs) | (y & b.m)) << b.bs); }
+__device__ __forceinline__ uint32_t cell_in_row(BrickShape b, int rank, uint32_t row, int x) { return ((uint32_t)rank << (3 * b.bs)) | row | (uint32_t)(x & b.m); }
+template <int kBS = 0>
+__device__ __forceinline__ uint32_t cell_slot(const GridDev& g, int rank, int x, int y, int z) {
+  const BrickShape b = brick_shape<kBS>(g);
+  return cell_in_row(b, rank, cell_row(b, y, z), x);
+}
+template <int kBS = 0>  // the cell of voxel (X, Y, Z) of the delta-field
+__device__ __forceinline__ uint32_t vox_cell(const GridDev& g, int rank, int X, int Y, int Z) { return cell_slot<kBS>(g, rank, X >> 2, Y >> 2, Z >> 2); }
+__device__ __forceinline__ const uint4* vox_cells(const uint32_t* vox) { return reinterpret_cast<const uint4*>(vox); }  // per slot
+// vox: word of voxel (X, Y, Z) in cell slot `cell` (one word per z-slab of the cell's 4x4x4 voxels) and the position of
+// the voxel's 2 bits in it (bit 0 MAYBE, bit 1 CERTAIN)
+__device__ __forceinline__ uint32_t vox_word(uint32_t cell, int Z) { return (cell << 2) | (uint32_t)(Z & 3); }
+__device__ __forceinline__ uint32_t vox_shift(int X, int Y) { return 2u * (uint32_t)(((Y & 3) << 2) | (X & 3)); }
+// boundary voxels (MAYBE, not CERTAIN) of a vox word: bit 2k set <=> voxel k is one
+__device__ __forceinline__ uint32_t boundary_bits(uint32_t w) { return w & ~(w >> 1) & 0x55555555u; }
+// vfine slot of the boundary voxel at shift `sh` of word `vz` (= w) of a cell whose 4 words are `cw`: vbase[cell]
+// (`base`, the boundary voxels of the cells before it in slot order) + the boundary voxels before it in bit order
+__device__ __forceinline__ uint32_t boundary_slot(uint32_t base, uint4 cw, uint32_t w, int vz, uint32_t sh) {
+  uint32_t slot = base + (uint32_t)__popc(boundary_bits(w) & ((1u << sh) - 1u));
+  slot += vz > 0 ? (uint32_t)__popc(boundary_bits(cw.x)) : 0u;
+  slot += vz > 1 ? (uint32_t)__popc(boundary_bits(cw.y)) : 0u;
+  slot += vz > 2 ? (uint32_t)__popc(boundary_bits(cw.z)) : 0u;
+  return slot;
+}
+// vfine[slot]: 16 bits per boundary voxel, MAYBE of child ch at bit ch, CERTAIN at bit 8 + ch; the child of the upper
+// half along x, y, z is bit 0, 1, 2 of ch (fine_child: of the position (fx, fy, fz) voxels above the low corner).  The
+// builder ORs into the 32-bit word fine_word(slot), at bit fine_half(slot).
+__device__ __forceinline__ uint32_t fine_child(float fx, float fy, float fz) { return (fx >= 0.5f ? 1u : 0u) | (fy >= 0.5f ? 2u : 0u) | (fz >= 0.5f ? 4u : 0u); }
+__device__ __forceinline__ uint32_t fine_maybe(int ch) { return 1u << ch; }
+__device__ __forceinline__ uint32_t fine_certain(int ch) { return 0x101u << ch; }   // CERTAIN implies MAYBE
+// bit 0 MAYBE, bit 1 CERTAIN, as in vox
+__device__ __forceinline__ uint32_t fine_state(uint32_t f, uint32_t ch) { return ((f >> ch) & 1u) | (((f >> (8u + ch)) & 1u) << 1); }
+__device__ __forceinline__ uint32_t fine_word(uint32_t slot) { return slot >> 1; }
+__device__ __forceinline__ uint32_t fine_half(uint32_t slot) { return (slot & 1u) * 16u; }
+// vocc: nibble of block origin cell slot `cell`; bit r: row (y0 + (r & 1), z0 + (r >> 1)) of the 2x2x2-cell block has points
+__device__ __forceinline__ uint32_t vocc_word(uint32_t cell) { return cell >> 3; }
+__device__ __forceinline__ uint32_t vocc_shift(uint32_t cell) { return (cell & 7u) * 4u; }
+
+// ---- warp helpers of the Morton-ordered query side
+// AABB of the warp's boxes: every lane ends with the union
+__device__ __forceinline__ void warp_aabb(float3& lo, float3& hi) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    lo.x = fminf(lo.x, __shfl_xor_sync(0xffffffffu, lo.x, o));
+    lo.y = fminf(lo.y, __shfl_xor_sync(0xffffffffu, lo.y, o));
+    lo.z = fminf(lo.z, __shfl_xor_sync(0xffffffffu, lo.z, o));
+    hi.x = fmaxf(hi.x, __shfl_xor_sync(0xffffffffu, hi.x, o));
+    hi.y = fmaxf(hi.y, __shfl_xor_sync(0xffffffffu, hi.y, o));
+    hi.z = fmaxf(hi.z, __shfl_xor_sync(0xffffffffu, hi.z, o));
+  }
+}
+// the 10 low bits of v spread to every third bit (one axis of a 30-bit Morton code)
+__device__ __forceinline__ uint32_t morton_spread10(uint32_t v) {
+  v = (v | (v << 16)) & 0x030000FFu;
+  v = (v | (v << 8)) & 0x0300F00Fu;
+  v = (v | (v << 4)) & 0x030C30C3u;
+  v = (v | (v << 2)) & 0x09249249u;
+  return v;
+}
 
 struct s4g_ctx {
   int device = 0;

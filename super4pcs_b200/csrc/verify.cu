@@ -106,28 +106,28 @@ __device__ __forceinline__ bool probe_run(const GridDev& g, uint32_t s, uint32_t
 template <bool kStats>
 __device__ __forceinline__ bool walk_row(const GridDev& g, int x0, int y0, int z0, int r, float tx, float ty,
                                          float tz, float sq_eps, ProbeStats& st) {
-  const int bs = g.bshift, m = (1 << bs) - 1;
+  const BrickShape b = brick_shape(g);
   const int xa = max(x0, 0), xb = min(x0 + 1, g.nx - 1);
-  const bool same_brick = (xa >> bs) == (xb >> bs);
+  const bool same_brick = brick_in_row(b, 0, xa) == brick_in_row(b, 0, xb);
   const int cz = z0 + (r >> 1), cy = y0 + (r & 1);
   bool found = false;
   if (cz >= 0 && cz < g.nz && cy >= 0 && cy < g.ny) {
-    const int rowb = ((cz >> bs) * g.tby + (cy >> bs)) * g.tbx;
-    const uint32_t rowl = (uint32_t)((((cz & m) << bs) | (cy & m)) << bs);
-    const int ra = __ldg(&g.top[rowb + (xa >> bs)]);
+    const int rowb = brick_row(g, b, cy, cz);
+    const uint32_t rowl = cell_row(b, cy, cz);
+    const int ra = __ldg(&g.top[brick_in_row(b, rowb, xa)]);
     if (kStats) st.bricks++;
     if (ra >= 0) {
-      const uint32_t idx = ((uint32_t)ra << (3 * bs)) | rowl | (uint32_t)(xa & m);
+      const uint32_t idx = cell_in_row(b, ra, rowl, xa);
       const uint32_t s = __ldg(&g.cellStart[idx]);
       const uint32_t e = __ldg(&g.cellStart[idx + (same_brick ? (uint32_t)(xb - xa) : 0u) + 1u]);
       if (kStats) st.ranges++;
       found = probe_run<kStats>(g, s, e, tx, ty, tz, sq_eps, st);
     }
     if (!same_brick && !found) {
-      const int rb = __ldg(&g.top[rowb + (xb >> bs)]);
+      const int rb = __ldg(&g.top[brick_in_row(b, rowb, xb)]);
       if (kStats) st.bricks++;
       if (rb >= 0) {
-        const uint32_t idx = ((uint32_t)rb << (3 * bs)) | rowl | (uint32_t)(xb & m);
+        const uint32_t idx = cell_in_row(b, rb, rowl, xb);
         const uint32_t s = __ldg(&g.cellStart[idx]);
         const uint32_t e = __ldg(&g.cellStart[idx + 1u]);
         if (kStats) st.ranges++;
@@ -145,11 +145,10 @@ __device__ __forceinline__ uint32_t block_rows(const GridDev& g, int x0, int y0,
   if (g.vocc != nullptr) {
     nib = 0u;
     if (x0 >= 0 && y0 >= 0 && z0 >= 0) {
-      const int bs = g.bshift, m = (1 << bs) - 1;
-      const int rank = __ldg(&g.vtop[((z0 >> bs) * g.tby + (y0 >> bs)) * g.tbx + (x0 >> bs)]);
+      const int rank = __ldg(&g.vtop[brick_index(g, x0, y0, z0)]);
       if (rank >= 0) {
-        const uint32_t cell = ((uint32_t)rank << (3 * bs)) | (uint32_t)((((z0 & m) << bs) | (y0 & m)) << bs) | (uint32_t)(x0 & m);
-        nib = (__ldg(&g.vocc[cell >> 3]) >> ((cell & 7u) * 4u)) & 0xFu;
+        const uint32_t cell = cell_slot(g, rank, x0, y0, z0);
+        nib = (__ldg(&g.vocc[vocc_word(cell)]) >> vocc_shift(cell)) & 0xFu;
       }
     }
   }
@@ -218,34 +217,13 @@ __device__ bool tile_live(const GridDev& g, const float* __restrict__ v, float4 
   return live;
 }
 
-// delta-field addressing of voxel (X,Y,Z) (bit 0 MAYBE, bit 1 CERTAIN; no v-brick = neither).  kBS > 0: brick shift
-// known at compile time (2 = the common 4x4x4-cell bricks), 0: read from the grid.
-template <int kBS>
-__device__ __forceinline__ int vtop_index(const GridDev& g, int X, int Y, int Z) {
-  const int bs = kBS > 0 ? kBS : g.bshift;
-  return ((Z >> (bs + 2)) * g.tby + (Y >> (bs + 2))) * g.tbx + (X >> (bs + 2));
-}
-// delta-field cell of voxel (X,Y,Z) inside v-brick `rank`, and the bit position of the voxel's 2 bits in its slab word
-template <int kBS>
-__device__ __forceinline__ uint32_t vox_cell(const GridDev& g, int rank, int X, int Y, int Z) {
-  const int bs = kBS > 0 ? kBS : g.bshift, m = (1 << bs) - 1;
-  return ((uint32_t)rank << (3 * bs)) | (uint32_t)(((((Z >> 2) & m) << bs) | ((Y >> 2) & m)) << bs | ((X >> 2) & m));
-}
-__device__ __forceinline__ uint32_t vox_shift(int X, int Y) { return 2u * (uint32_t)(((Y & 3) << 2) | (X & 3)); }
-
 // second level: state of the sub-voxel (edge h/8) of boundary voxel (X,Y,Z) that holds the position (ux,uy,uz); w = the
-// voxel's slab word, sh = its bit position (GridDev::vfine: slot = the cell's base + the boundary voxels before it)
+// voxel's slab word, sh = its bit position
 __device__ __forceinline__ uint32_t vox_refine(const GridDev& g, uint32_t cell, uint32_t w, uint32_t sh, int X, int Y, int Z, float ux,
                                                float uy, float uz) {
-  const uint4 cw = __ldg(reinterpret_cast<const uint4*>(g.vox) + cell);
-  const int vz = Z & 3;
-  uint32_t slot = __ldg(&g.vbase[cell]) + (uint32_t)__popc((w & ~(w >> 1) & 0x55555555u) & ((1u << sh) - 1u));
-  slot += vz > 0 ? (uint32_t)__popc(cw.x & ~(cw.x >> 1) & 0x55555555u) : 0u;
-  slot += vz > 1 ? (uint32_t)__popc(cw.y & ~(cw.y >> 1) & 0x55555555u) : 0u;
-  slot += vz > 2 ? (uint32_t)__popc(cw.z & ~(cw.z >> 1) & 0x55555555u) : 0u;
-  const uint32_t f = __ldg(&g.vfine[slot]);
-  const uint32_t ch = ((ux - (float)X) >= 0.5f ? 1u : 0u) | ((uy - (float)Y) >= 0.5f ? 2u : 0u) | ((uz - (float)Z) >= 0.5f ? 4u : 0u);
-  return ((f >> ch) & 1u) | (((f >> (8u + ch)) & 1u) << 1);
+  const uint4 cw = __ldg(vox_cells(g.vox) + cell);
+  const uint32_t f = __ldg(&g.vfine[boundary_slot(__ldg(&g.vbase[cell]), cw, w, Z & 3, sh)]);
+  return fine_state(f, fine_child(ux - (float)X, uy - (float)Y, uz - (float)Z));
 }
 
 // state of the voxel (X,Y,Z) = floor of the voxel-space position (ux,uy,uz): bit 0 MAYBE, bit 1 CERTAIN; a BOUNDARY voxel
@@ -253,7 +231,7 @@ __device__ __forceinline__ uint32_t vox_refine(const GridDev& g, uint32_t cell, 
 template <int kBS>
 __device__ __forceinline__ uint32_t vox_state(const GridDev& g, int rank, int X, int Y, int Z, float ux, float uy, float uz) {
   const uint32_t cell = vox_cell<kBS>(g, rank, X, Y, Z), sh = vox_shift(X, Y);
-  const uint32_t w = __ldg(&g.vox[(cell << 2) | (uint32_t)(Z & 3)]);
+  const uint32_t w = __ldg(&g.vox[vox_word(cell, Z)]);
   uint32_t s = (w >> sh) & 3u;
   if (S4G_SUBVOXEL && s == 1u && g.vfine != nullptr) s = vox_refine(g, cell, w, sh, X, Y, Z, ux, uy, uz);
   return s;
@@ -382,14 +360,14 @@ k_verify(GridDev g, const float4* __restrict__ Q, const float4* __restrict__ til
         const int bX = __float2int_rd(bx), bY = __float2int_rd(by), bZ = __float2int_rd(bz);
         const bool ina = (uint32_t)aX < lx && (uint32_t)aY < limY && (uint32_t)aZ < limZ;
         const bool inb = two && (uint32_t)bX < lx && (uint32_t)bY < limY && (uint32_t)bZ < limZ;
-        const int ra = ina ? __ldg(&g.vtop[vtop_index<kBS>(g, aX, aY, aZ)]) : -1;
-        const int rb = inb ? __ldg(&g.vtop[vtop_index<kBS>(g, bX, bY, bZ)]) : -1;
+        const int ra = ina ? __ldg(&g.vtop[brick_index<kBS, 2>(g, aX, aY, aZ)]) : -1;
+        const int rb = inb ? __ldg(&g.vtop[brick_index<kBS, 2>(g, bX, bY, bZ)]) : -1;
         if (kStats) st.bitmap += (ina ? 1 : 0) + (inb ? 1 : 0);
         if ((ra & rb) >= 0) {                        // some lane of the warp landed in a v-brick (for a or for b): both words in flight
           const uint32_t cella = vox_cell<kBS>(g, ra, aX, aY, aZ), cellb = vox_cell<kBS>(g, rb, bX, bY, bZ);
           const uint32_t sha = vox_shift(aX, aY), shb = vox_shift(bX, bY);
-          const uint32_t wa = ra >= 0 ? __ldg(&g.vox[(cella << 2) | (uint32_t)(aZ & 3)]) : 0u;
-          const uint32_t wb = rb >= 0 ? __ldg(&g.vox[(cellb << 2) | (uint32_t)(bZ & 3)]) : 0u;
+          const uint32_t wa = ra >= 0 ? __ldg(&g.vox[vox_word(cella, aZ)]) : 0u;
+          const uint32_t wb = rb >= 0 ? __ldg(&g.vox[vox_word(cellb, bZ)]) : 0u;
           uint32_t sa = (wa >> sha) & 3u, sb = (wb >> shb) & 3u;
           if (kStats) st.bitmap += (ra >= 0 ? 1 : 0) + (rb >= 0 ? 1 : 0);
           if (S4G_SUBVOXEL && g.vfine != nullptr) {
@@ -416,7 +394,7 @@ k_verify(GridDev g, const float4* __restrict__ Q, const float4* __restrict__ til
         else voxel_of<false>(g, &sV[c * 12], nullptr, q, ux, uy, uz);
         const bool in = valid && ux >= 0.f && uy >= 0.f && uz >= 0.f && ux < (float)limX && uy < (float)limY && uz < (float)limZ;
         const int X = in ? __float2int_rd(ux) : 0, Y = in ? __float2int_rd(uy) : 0, Z = in ? __float2int_rd(uz) : 0;
-        const int r = in ? __ldg(&g.vtop[vtop_index<kBS>(g, X, Y, Z)]) : -1;
+        const int r = in ? __ldg(&g.vtop[brick_index<kBS, 2>(g, X, Y, Z)]) : -1;
         if (kStats) st.bitmap += in ? 1 : 0;
         if (r >= 0) {
           const uint32_t sa = vox_state<kBS>(g, r, X, Y, Z, ux, uy, uz);
@@ -513,14 +491,6 @@ __global__ void k_pack_rec(const float* __restrict__ T16, int K, VerifyRecArgs r
   s4g_verify_record(m, ra, &recs[k]);
 }
 
-__device__ __forceinline__ uint32_t spread10(uint32_t v) {
-  v = (v | (v << 16)) & 0x030000FFu;
-  v = (v | (v << 8)) & 0x0300F00Fu;
-  v = (v | (v << 4)) & 0x030C30C3u;
-  v = (v | (v << 2)) & 0x09249249u;
-  return v;
-}
-
 // One thread per candidate, when the candidates are ordered per query patch: the sort key of every (patch, candidate)
 // pair: patch << 32 | beyond the device-side count << 31 | robust path << 30 | 30-bit Morton code of T c_patch in cell
 // coordinates (scaled by `mscale` to 10 bits per axis).  Candidates beyond the count sort last in every patch, so the
@@ -543,7 +513,7 @@ __global__ void k_verify_keys(const VerifyCand* __restrict__ recs, int K, const 
       const uint32_t ux = (uint32_t)min(1023, max(0, __float2int_rd(x)));
       const uint32_t uy = (uint32_t)min(1023, max(0, __float2int_rd(y)));
       const uint32_t uz = (uint32_t)min(1023, max(0, __float2int_rd(z)));
-      code = spread10(ux) | (spread10(uy) << 1) | (spread10(uz) << 2);
+      code = morton_spread10(ux) | (morton_spread10(uy) << 1) | (morton_spread10(uz) << 2);
     }
     keys[(size_t)p * K + k] = (unsigned long long)p << 32 | code;
     vals[(size_t)p * K + k] = (uint32_t)k;
@@ -560,15 +530,7 @@ __global__ void k_patch_centres(const float4* __restrict__ tiles, int nTiles, in
     lo.x = fminf(lo.x, s.x - s.w); lo.y = fminf(lo.y, s.y - s.w); lo.z = fminf(lo.z, s.z - s.w);
     hi.x = fmaxf(hi.x, s.x + s.w); hi.y = fmaxf(hi.y, s.y + s.w); hi.z = fmaxf(hi.z, s.z + s.w);
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    lo.x = fminf(lo.x, __shfl_xor_sync(0xffffffffu, lo.x, o));
-    lo.y = fminf(lo.y, __shfl_xor_sync(0xffffffffu, lo.y, o));
-    lo.z = fminf(lo.z, __shfl_xor_sync(0xffffffffu, lo.z, o));
-    hi.x = fmaxf(hi.x, __shfl_xor_sync(0xffffffffu, hi.x, o));
-    hi.y = fmaxf(hi.y, __shfl_xor_sync(0xffffffffu, hi.y, o));
-    hi.z = fmaxf(hi.z, __shfl_xor_sync(0xffffffffu, hi.z, o));
-  }
+  warp_aabb(lo, hi);
   if (lane == 0) out[p] = make_float4(0.5f * (lo.x + hi.x), 0.5f * (lo.y + hi.y), 0.5f * (lo.z + hi.z), 0.f);
 }
 
