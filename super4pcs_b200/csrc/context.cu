@@ -275,18 +275,18 @@ __global__ void k_gather_f4(const float4* __restrict__ src, const uint32_t* __re
   dst[i] = src[idx[i]];
 }
 
-// ---- delta-field (see GridDev::vox): v-bricks = bricks within `reach` of a P point (the 8 corners of the box
-// p +- reach suffice: reach < one cell, a brick is >= 4 cells wide)
+// ---- delta-field (see GridDev::vox): v-bricks = bricks within `reach` of a P point: every brick the box p +- reach
+// touches.  For centred clouds reach is below one cell and these are the bricks of the box's 8 corners; far from the
+// origin the field's slack grows with the coordinates and the box can span several bricks per axis.
 __global__ void k_mark_vbricks(GridDev g, const float4* __restrict__ P, int n, float reach, int* __restrict__ vtop) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   float4 p = P[i];
-#pragma unroll
-  for (int d = 0; d < 8; ++d) {
-    int3 c = cell_of(g, p.x + ((d & 1) ? reach : -reach), p.y + ((d & 2) ? reach : -reach),
-                     p.z + ((d & 4) ? reach : -reach));
-    vtop[brick_index(g, c.x, c.y, c.z)] = 1;
-  }
+  const int3 a = cell_of(g, p.x - reach, p.y - reach, p.z - reach), b = cell_of(g, p.x + reach, p.y + reach, p.z + reach);
+  const int bs = g.bshift;
+  for (int z = a.z >> bs; z <= b.z >> bs; ++z)
+    for (int y = a.y >> bs; y <= b.y >> bs; ++y)
+      for (int x = a.x >> bs; x <= b.x >> bs; ++x) vtop[brick_index(g, x << bs, y << bs, z << bs)] = 1;
   // ... and the origin cells c - (dx, dy, dz) of the 2x2x2 blocks that contain the point's cell (GridDev::vocc lives there)
   const int3 c = cell_of(g, p.x, p.y, p.z);
 #pragma unroll

@@ -190,11 +190,13 @@ __device__ bool tile_live(const GridDev& g, const float* __restrict__ v, float4 
   // single exit, flag based (see DESIGN.md section 7 on early returns + warp votes)
   bool live = true;
   if (g.csat != nullptr) {
-    // centre in cell coordinates, radius in cells: r/h + delta/h (< 0.4951) + slack
+    // centre in cell coordinates, radius in cells: r/h + delta/h (< 0.4951) + the rounding of the centre.  The centre comes
+    // from the same FMA chain as a fast-path voxel, so its error is within the candidate's bound E <= vslack (world units,
+    // s4g_verify_record): 0.52 cells cover it for centred clouds, and vslack / h, which grows with |coordinates|, beyond
     const float cx = 0.25f * __fmaf_rn(v[0], sph.x, __fmaf_rn(v[1], sph.y, __fmaf_rn(v[2], sph.z, v[3])));
     const float cy = 0.25f * __fmaf_rn(v[4], sph.x, __fmaf_rn(v[5], sph.y, __fmaf_rn(v[6], sph.z, v[7])));
     const float cz = 0.25f * __fmaf_rn(v[8], sph.x, __fmaf_rn(v[9], sph.y, __fmaf_rn(v[10], sph.z, v[11])));
-    const float R = sph.w * g.inv_h * scale * 1.0001f + 0.52f;
+    const float R = sph.w * g.inv_h * scale * 1.0001f + fmaxf(0.52f, 0.5f + g.vslack * g.inv_h * 1.0001f);
     const float fx0 = cx - R, fx1 = cx + R, fy0 = cy - R, fy1 = cy + R, fz0 = cz - R, fz1 = cz + R;
     // boxes entirely outside the grid cannot match anything
     const bool inside = fx1 >= 0.f && fy1 >= 0.f && fz1 >= 0.f && fx0 < (float)g.nx && fy0 < (float)g.ny &&
