@@ -9,6 +9,7 @@
 #include "super4pcs/algorithms/match4pcsBase.h"
 
 #include <algorithm>
+#include <chrono>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
@@ -127,11 +128,6 @@ Match4PCSBase::~Match4PCSBase() {
   gpu_ = nullptr;
 }
 
-void Match4PCSBase::ThrowDeviceError(const char* where) const {
-  throw std::runtime_error(std::string("super4pcs-b200: ") + where + ": " +
-                           (gpu_ ? s4g_error_string(gpu_) : "no CUDA device (there is no CPU fallback)"));
-}
-
 void Match4PCSBase::ThrowLaneError(const s4g_ctx* lane, const char* where) const {
   throw std::runtime_error(std::string("super4pcs-b200: ") + where + ": " +
                            (lane ? s4g_error_string(lane) : "no CUDA device (there is no CPU fallback)"));
@@ -141,7 +137,7 @@ void Match4PCSBase::EnsureDevice() const {
   if (gpu_) return;
   if (s4g_create(devices_[0], &gpu_) != S4G_OK) {
     gpu_ = nullptr;
-    ThrowDeviceError("s4g_create");
+    ThrowLaneError(nullptr, "s4g_create");
   }
 }
 
@@ -378,50 +374,57 @@ Match4PCSBase::Scalar Match4PCSBase::Verify(const Eigen::Ref<const MatrixType>& 
   EnsureDevice();
   const MatrixType T = mat;  // contiguous column-major copy
   uint32_t count = 0;
-  if (s4g_verify(gpu_, T.data(), 1, &count) != S4G_OK) ThrowDeviceError("s4g_verify");
+  if (s4g_verify(gpu_, T.data(), 1, &count) != S4G_OK) ThrowLaneError(gpu_, "s4g_verify");
   return Scalar(count) / Scalar(sampled_Q_3D_.size());
 }
 
-bool Match4PCSBase::TryBaseOnDevice(Scalar, Scalar, Scalar, Scalar, Scalar, Scalar, const int*, DeviceBest*) {
-  return false;
+bool Match4PCSBase::TryBaseOnLane(s4g_ctx*, const SelectedBase&, DeviceBest*) const { return false; }
+
+bool Match4PCSBase::TryBasesOnLane(s4g_ctx*, const std::vector<SelectedBase*>&) const { return false; }
+
+void Match4PCSBase::SelectBase(SelectedBase* sb) {
+  const std::chrono::steady_clock::time_point t_sel = std::chrono::steady_clock::now();
+  sb->selected = SelectQuadrilateral(sb->invariant1, sb->invariant2, sb->ids[0], sb->ids[1], sb->ids[2], sb->ids[3]);
+  if (timings_) stats_.ms_select += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_sel).count();
+  if (sb->selected) {
+    sb->distance1 = (base_3D_[0].pos() - base_3D_[1].pos()).norm();
+    sb->distance2 = (base_3D_[2].pos() - base_3D_[3].pos()).norm();
+    sb->normal_angle1 = (base_3D_[0].normal() - base_3D_[1].normal()).norm();
+    sb->normal_angle2 = (base_3D_[2].normal() - base_3D_[3].normal()).norm();
+    sb->base3d = base_3D_;
+    PrepareBaseOrder(sb->distance1, sb->distance2, &sb->order);
+  }
+  sb->rng_after = randomGenerator_;
 }
 
-bool Match4PCSBase::TryBasesOnLane(s4g_ctx*, const std::vector<SpeculativeBase*>&) const { return false; }
-
-bool Match4PCSBase::TryBaseOnLane(s4g_ctx*, const std::vector<Point3D>&, Scalar, Scalar, Scalar, Scalar, Scalar,
-                                  Scalar, const int*, DeviceBest*) const {
-  return false;
-}
-
-// Row f1.  Runs every selected base of spec_ through TryBaseOnLane, base k on lane k (lane 0 = gpu_
-// on the calling thread, the others on one short-lived thread each: a base is a chain of stream
-// launches with blocking size read-backs, so host threads are what lets the chains overlap).
+// Row f1.  Runs the selected bases of spec_: in one launch chain on gpu_ when batches are on and several bases were
+// selected ahead, else each through TryBaseOnLane, base k on lane k (lane 0 = gpu_ on the calling thread, the others
+// on one short-lived thread each: a base is a chain of stream launches with blocking size read-backs, so host threads
+// are what lets the chains overlap).  One base selected: the per-base chain on gpu_.
 void Match4PCSBase::RunSpeculation() {
   EnsureDevice();
-  size_t selected = 0;
-  for (const SpeculativeBase& sb : spec_) selected += sb.selected ? 1 : 0;
-  if (BatchOn() && selected > 0) {
+  std::vector<SelectedBase*> selected;
+  for (SelectedBase& sb : spec_)  // (deque elements do not move while nothing is inserted)
+    if (sb.selected) selected.push_back(&sb);
+  auto run = [this](SelectedBase* sb, s4g_ctx* lane) {
+    sb->lane = lane;
+    try {
+      sb->handled = TryBaseOnLane(lane, *sb, &sb->best);
+    } catch (...) {
+      sb->error = std::current_exception();
+    }
+  };
+  if (BatchOn() && spec_.size() > 1) {
     // one launch chain for all the selected bases (s4g_try_bases); candidate sharding over several devices keeps the
     // per-base chain (its quads have to be resident on every device)
-    std::vector<SpeculativeBase*> list;
-    for (SpeculativeBase& sb : spec_)
-      if (sb.selected) list.push_back(&sb);
-    if (TryBasesOnLane(gpu_, list)) return;
+    if (TryBasesOnLane(gpu_, selected)) return;
     if (lane_count_ <= 1) {  // no batched pass for this matcher and no lanes: one base after the other on the primary context
-      for (SpeculativeBase* sb : list) {
-        sb->lane = gpu_;
-        try {
-          sb->handled = TryBaseOnLane(gpu_, sb->base3d, sb->invariant1, sb->invariant2, sb->distance1, sb->distance2,
-                                      sb->normal_angle1, sb->normal_angle2, sb->ids, &sb->best);
-        } catch (...) {
-          sb->error = std::current_exception();
-        }
-      }
+      for (SelectedBase* sb : selected) run(sb, gpu_);
       return;
     }
   }
-  if (selected > 1) {
-    while (lanes_.size() + 1 < selected) {
+  if (selected.size() > 1) {
+    while (lanes_.size() + 1 < selected.size()) {
       s4g_ctx* lane = nullptr;
       if (s4g_create(devices_[0], &lane) != S4G_OK) ThrowLaneError(nullptr, "s4g_create (lane)");
       lanes_.push_back(lane);
@@ -434,26 +437,11 @@ void Match4PCSBase::RunSpeculation() {
   }
   if (devices_.size() > 1) {  // every lane that runs below shards its candidates over the other devices
     PreparePeers(gpu_);
-    for (size_t k = 0; k + 1 < selected && k < lanes_.size(); ++k) PreparePeers(lanes_[k]);
+    for (size_t k = 0; k + 1 < selected.size() && k < lanes_.size(); ++k) PreparePeers(lanes_[k]);
   }
-  auto run = [this](SpeculativeBase* sb, s4g_ctx* lane) {
-    sb->lane = lane;
-    try {
-      sb->handled = TryBaseOnLane(lane, sb->base3d, sb->invariant1, sb->invariant2, sb->distance1, sb->distance2,
-                                  sb->normal_angle1, sb->normal_angle2, sb->ids, &sb->best);
-    } catch (...) {
-      sb->error = std::current_exception();
-    }
-  };
   std::vector<std::thread> workers;
-  SpeculativeBase* mine = nullptr;
-  size_t next_lane = 0;
-  for (SpeculativeBase& sb : spec_) {  // (deque elements do not move while nothing is inserted)
-    if (!sb.selected) continue;
-    if (mine == nullptr) mine = &sb;
-    else workers.emplace_back(run, &sb, lanes_[next_lane++]);
-  }
-  if (mine != nullptr) run(mine, gpu_);
+  for (size_t k = 1; k < selected.size(); ++k) workers.emplace_back(run, selected[k], lanes_[k - 1]);
+  if (!selected.empty()) run(selected[0], gpu_);
   for (std::thread& w : workers) w.join();
 }
 

@@ -49,7 +49,7 @@ void MatchSuper4PCS::Initialize(const std::vector<Point3D>&, const std::vector<P
   if (!exact_order_ || sampled_Q_3D_.empty() || sampled_Q_3D_.size() > kMaxPoints) return;
   EnsureDevice();
   float norm[5];
-  if (s4g_get_q_normalization(gpu_, norm) != S4G_OK) ThrowDeviceError("s4g_get_q_normalization");
+  if (s4g_get_q_normalization(gpu_, norm) != S4G_OK) ThrowLaneError(gpu_, "s4g_get_q_normalization");
   std::vector<float> unit(3 * sampled_Q_3D_.size());
   for (size_t i = 0; i < sampled_Q_3D_.size(); ++i)
     for (int c = 0; c < 3; ++c) unit[3 * i + size_t(c)] = (sampled_Q_3D_[i].pos()[c] - norm[c]) / norm[3] + 0.5f;  // worldToUnit
@@ -135,11 +135,11 @@ void MatchSuper4PCS::ExtractPairs(Scalar pair_distance, Scalar pair_normals_angl
   const s4g_pair_filters f = Filters(options_);
   int64_t n = 0;
   if (s4g_extract_pairs(gpu_, pair_distance, pair_normals_angle, pair_distance_epsilon, b1, b2, &f, 0, &n) != S4G_OK)
-    ThrowDeviceError("s4g_extract_pairs");
+    ThrowLaneError(gpu_, "s4g_extract_pairs");
   static_assert(sizeof(std::pair<int, int>) == 2 * sizeof(int), "pair<int,int> must be two packed ints");
   pairs->resize(size_t(n));
   if (n > 0 && s4g_get_pairs(gpu_, 0, reinterpret_cast<int32_t*>(pairs->data())) != S4G_OK)
-    ThrowDeviceError("s4g_get_pairs");
+    ThrowLaneError(gpu_, "s4g_get_pairs");
   if (order_) {  // S4PCS_EXACT_ORDER: hand the list over in the reference's emission order instead of sorted
     std::vector<uint32_t> pos;
     order_->Replay(pair_distance, pair_distance_epsilon, &pos);
@@ -158,42 +158,30 @@ bool MatchSuper4PCS::FindCongruentQuadrilaterals(Scalar invariant1, Scalar invar
   EnsureDevice();
   if (s4g_set_pairs(gpu_, 0, reinterpret_cast<const int32_t*>(P_pairs.data()), int64_t(P_pairs.size())) != S4G_OK ||
       s4g_set_pairs(gpu_, 1, reinterpret_cast<const int32_t*>(Q_pairs.data()), int64_t(Q_pairs.size())) != S4G_OK)
-    ThrowDeviceError("s4g_set_pairs");
+    ThrowLaneError(gpu_, "s4g_set_pairs");
   float base_xyz[12];
   for (int k = 0; k < 4; ++k)
     for (int c = 0; c < 3; ++c) base_xyz[3 * k + c] = base_3D_[k].pos()[c];
   int64_t n = 0;
   if (s4g_find_quads(gpu_, invariant1, invariant2, distance_threshold2, base_xyz, &n) != S4G_OK)
-    ThrowDeviceError("s4g_find_quads");
+    ThrowLaneError(gpu_, "s4g_find_quads");
   quadrilaterals->assign(size_t(n), Quadrilateral(0, 0, 0, 0));
   if (n > 0 && s4g_get_quads(gpu_, quadrilaterals->front().vertices.data()) != S4G_OK)
-    ThrowDeviceError("s4g_get_quads");
+    ThrowLaneError(gpu_, "s4g_get_quads");
   return !quadrilaterals->empty();
 }
 
-bool MatchSuper4PCS::TryBaseOnDevice(Scalar invariant1, Scalar invariant2, Scalar distance1, Scalar distance2,
-                                     Scalar normal_angle1, Scalar normal_angle2, const int base_ids[4],
-                                     DeviceBest* out) {
-  if (!fused_) return false;
-  EnsureDevice();
-  PreparePeers(gpu_);  // S4PCS_DEVICES: the contexts on the other devices (no-op with one device)
-  return TryBaseOnLane(gpu_, base_3D_, invariant1, invariant2, distance1, distance2, normal_angle1, normal_angle2,
-                       base_ids, out);
-}
-
-bool MatchSuper4PCS::TryBaseOnLane(s4g_ctx* lane, const std::vector<Point3D>& base3d, Scalar invariant1,
-                                   Scalar invariant2, Scalar distance1, Scalar distance2, Scalar normal_angle1,
-                                   Scalar normal_angle2, const int base_ids[4], DeviceBest* out) const {
+bool MatchSuper4PCS::TryBaseOnLane(s4g_ctx* lane, const SelectedBase& base, DeviceBest* out) const {
   if (!fused_) return false;
   const Scalar eps = distance_factor * options_.delta;
   const s4g_pair_filters f = Filters(options_);
   float b[4][9];
-  for (int k = 0; k < 4; ++k) Point9(base3d[k], b[k]);
+  for (int k = 0; k < 4; ++k) Point9(base.base3d[k], b[k]);
   float base_xyz[12], basep_xyz[12];  // TryCongruentSet works on sampled_P[base ids] (== base3d after the reordering)
   for (int k = 0; k < 4; ++k)
     for (int c = 0; c < 3; ++c) {
-      base_xyz[3 * k + c] = base3d[k].pos()[c];
-      basep_xyz[3 * k + c] = sampled_P_3D_[base_ids[k]].pos()[c];
+      base_xyz[3 * k + c] = base.base3d[k].pos()[c];
+      basep_xyz[3 * k + c] = sampled_P_3D_[base.ids[k]].pos()[c];
     }
   // One pass per device context (S4PCS_DEVICES; a single one by default): pairs and quads are replicated, the
   // candidates of TryCongruentSet are sharded by quad index (SURVEY.md section 8, row e; cpp/shards.h).
@@ -209,17 +197,17 @@ bool MatchSuper4PCS::TryBaseOnLane(s4g_ctx* lane, const std::vector<Point3D>& ba
   detail::ForEachShard(lane, peers, [&](s4g_ctx* ctx, int rank, int world) {
     Pass& p = pass[size_t(rank)];
     const bool timed = timings_ && rank == 0;  // S4PCS_TIMINGS: the events of the context that also holds the result
-    if (s4g_extract_pairs(ctx, distance1, normal_angle1, eps, b[0], b[1], &f, 0, &p.n1) != S4G_OK)
+    if (s4g_extract_pairs(ctx, base.distance1, base.normal_angle1, eps, b[0], b[1], &f, 0, &p.n1) != S4G_OK)
       ThrowLaneError(ctx, "s4g_extract_pairs");
     if (timed && s4g_get_timings(ctx, p.ms) == S4G_OK) p.ms_pairs1 = p.ms[2];  // (the slot-1 call re-uses the event pair)
-    if (s4g_extract_pairs(ctx, distance2, normal_angle2, eps, b[2], b[3], &f, 1, &p.n2) != S4G_OK)
+    if (s4g_extract_pairs(ctx, base.distance2, base.normal_angle2, eps, b[2], b[3], &f, 1, &p.n2) != S4G_OK)
       ThrowLaneError(ctx, "s4g_extract_pairs");
     struct ReadTimings {  // on every way out of this pass
       s4g_ctx* ctx; Pass* p; bool on;
       ~ReadTimings() { if (on) (void)s4g_get_timings(ctx, p->ms); }
     } read_timings{ctx, &p, timed};
     if (p.n1 == 0 || p.n2 == 0) return;
-    if (s4g_find_quads(ctx, invariant1, invariant2, eps, base_xyz, &p.nq) != S4G_OK) ThrowLaneError(ctx, "s4g_find_quads");
+    if (s4g_find_quads(ctx, base.invariant1, base.invariant2, eps, base_xyz, &p.nq) != S4G_OK) ThrowLaneError(ctx, "s4g_find_quads");
     if (p.nq == 0) return;
     if (gated && !gate.Pass(rank)) return;  // a peer left early: its error (or the count check below) reports it
     if (s4g_try_congruent_set_resident(ctx, basep_xyz, options_.max_angle, eps, rank, world, &p.r) != S4G_OK)
@@ -249,13 +237,13 @@ bool MatchSuper4PCS::TryBaseOnLane(s4g_ctx* lane, const std::vector<Point3D>& ba
 
 // Row f1, single-launch form: the whole per-base chain of TryBaseOnLane for every base of `bases` in one call of
 // s4g_try_bases (base index = grid dimension / key prefix, three read-backs per batch).  Same results per base.
-bool MatchSuper4PCS::TryBasesOnLane(s4g_ctx* lane, const std::vector<SpeculativeBase*>& bases) const {
+bool MatchSuper4PCS::TryBasesOnLane(s4g_ctx* lane, const std::vector<SelectedBase*>& bases) const {
   if (!fused_ || bases.empty() || bases.size() > 64) return false;
   const Scalar eps = distance_factor * options_.delta;
   const s4g_pair_filters f = Filters(options_);
   std::vector<s4g_base_desc> desc(bases.size());
   for (size_t b = 0; b < bases.size(); ++b) {
-    const SpeculativeBase& sb = *bases[b];
+    const SelectedBase& sb = *bases[b];
     s4g_base_desc& d = desc[b];
     d.pair_distance[0] = sb.distance1;
     d.pair_distance[1] = sb.distance2;
@@ -275,7 +263,7 @@ bool MatchSuper4PCS::TryBasesOnLane(s4g_ctx* lane, const std::vector<Speculative
   if (rc == S4G_ERR_ARG || rc == S4G_ERR_NOMEM) return false;
   if (rc != S4G_OK) ThrowLaneError(lane, "s4g_try_bases");
   for (size_t b = 0; b < bases.size(); ++b) {
-    SpeculativeBase& sb = *bases[b];
+    SelectedBase& sb = *bases[b];
     const s4g_base_result& r = res[b];
     DeviceBest& out = sb.best;
     out = DeviceBest();

@@ -159,17 +159,6 @@ class Match4PCSBase {
     /// the winner and the counts of a TryCongruentSet result record; the pair / quad counts and stage times stay as they are
     void SetFrom(const s4g_tcs_result& r);
   };
-  /// One fused pass pairs -> quads -> rigid fit -> Verify entirely on the device.  The base
-  /// implementation reports "unsupported" (returns false) so that subclasses providing only
-  /// the three virtual stages still work through the generic path.
-  virtual bool TryBaseOnDevice(Scalar invariant1, Scalar invariant2, Scalar distance1, Scalar distance2,
-                               Scalar normal_angle1, Scalar normal_angle2, const int base_ids[4], DeviceBest* out);
-  /// The same pass for an explicit base on an explicit device context.  Reads only immutable
-  /// state (options_, sampled_P_3D_), so several lanes may run it concurrently from different
-  /// threads, each on its own context.
-  virtual bool TryBaseOnLane(s4g_ctx* lane, const std::vector<Point3D>& base3d, Scalar invariant1,
-                             Scalar invariant2, Scalar distance1, Scalar distance2, Scalar normal_angle1,
-                             Scalar normal_angle2, const int base_ids[4], DeviceBest* out) const;
   /// The ORDER in which the reference would have seen the two pair lists of a base (it does not sort them, its
   /// candidate order -- and the winner among candidates with equal inlier counts -- follows from it; cpp/pair_order.h).
   /// Empty (valid == false) unless a subclass replays that order (MatchSuper4PCS with S4PCS_EXACT_ORDER=1).
@@ -190,7 +179,6 @@ class Match4PCSBase {
   void AdoptIfBetter(const int base_ids[4], const DeviceBest& b);
   void EnsureDevice() const;                       ///< creates gpu_ (throws std::runtime_error)
   void UploadClouds();                             ///< sampled_P/Q -> device (grid, Morton copy, unit cube)
-  [[noreturn]] void ThrowDeviceError(const char* where) const;
   [[noreturn]] void ThrowLaneError(const s4g_ctx* lane, const char* where) const;
   void UploadCloudsTo(s4g_ctx* ctx) const;
   void UploadCloudsToAll(const std::vector<s4g_ctx*>& contexts) const;  ///< concurrently, one host thread per context
@@ -215,19 +203,20 @@ class Match4PCSBase {
   void AccountBase(const DeviceBest& b);
   void LogTimings() const;
 
-  // ---- speculative multi-base execution (SURVEY.md section 8, row f1)
+  // ---- bases selected ahead (SURVEY.md section 8, row f1)
   // The reference tries one base at a time (hpp:236-256); a small sample keeps a GPU idle that
   // way (a base is a handful of tiny kernels and size read-backs).  Base selection depends only on
   // the RNG and on sampled P, and a base's best candidate does not depend on best_LCP_ (hpp:363-497
-  // verifies every gate-passing quad), so the next few bases are selected ahead -- in RNG order --
-  // and run concurrently, one device context ("lane") and one host thread each.  Results are
-  // consumed strictly in order, with the reference's adoption and termination checks between
-  // bases; bases selected beyond the terminating one are discarded and the RNG is put back to the
-  // state right after the last consumed base, so that every observable (result, visitor calls,
-  // RNG, base_3D_) is what the sequential loop produces.  Lanes: S4PCS_LANES (default 1 = off).
-  struct SpeculativeBase {
+  // verifies every gate-passing quad), so TryOneBase selects `depth` bases ahead in RNG order, runs
+  // them -- one device context ("lane") and one host thread each (S4PCS_LANES, default 1 = off), or
+  // one launch chain (S4PCS_BATCH); at depth one, the reference's loop, the per-base chain on gpu_ --
+  // and consumes them strictly in order with the reference's adoption and termination checks between
+  // bases.  Bases selected beyond the terminating one are discarded and the RNG is put back to the
+  // state right after the last consumed base, so that every observable (result, visitor calls, RNG,
+  // base_3D_) is the same at any depth.
+  struct SelectedBase {
     bool selected = false;   ///< SelectQuadrilateral succeeded
-    bool handled = false;    ///< the fused device pass ran (else: generic path when consumed)
+    bool handled = false;    ///< the fused device pass ran (else: the three virtual stages when consumed)
     Scalar invariant1 = 0, invariant2 = 0, distance1 = 0, distance2 = 0, normal_angle1 = 0, normal_angle2 = 0;
     int ids[4] = {0, 0, 0, 0};
     std::vector<Point3D> base3d;
@@ -238,9 +227,9 @@ class Match4PCSBase {
     bool batched = false;     ///< ran inside one s4g_try_bases launch chain: the lane holds no resident lists of this base
     std::exception_ptr error;
   };
-  std::deque<SpeculativeBase> spec_;
-  std::mt19937 rng_consumed_;            ///< RNG state after the last consumed speculative base
-  BaseOrder order_consumed_;             ///< pair-order replay state after the last consumed speculative base
+  std::deque<SelectedBase> spec_;        ///< selected, not yet consumed
+  std::mt19937 rng_consumed_;            ///< RNG state after the last consumed base
+  BaseOrder order_consumed_;             ///< pair-order replay state after the last consumed base
   int spec_budget_ = 1;                  ///< bases the current Perform_N_steps call may still try
   int lane_count_ = 1;
   // Bases per launch chain (s4g_try_bases): S4PCS_BATCH = the maximum (default 32, 1 = off).  Used while the sampled Q cloud
@@ -258,15 +247,24 @@ class Match4PCSBase {
     batch_now_ = std::min(batch_, 2 * batch_now_);
     return d;
   }
+  /// One fused pass pairs -> quads -> rigid fit -> Verify of `base` entirely on the context `lane`; false (the default):
+  /// no fused pass, the base goes through the three virtual stages.  Reads only immutable state (options_,
+  /// sampled_P_3D_), so several lanes may run it concurrently from different threads, each on its own context.
+  virtual bool TryBaseOnLane(s4g_ctx* lane, const SelectedBase& base, DeviceBest* out) const;
   /// Runs every base of `bases` (selected ahead, in RNG order) in ONE device launch chain on `lane`; fills handled / best /
-  /// batched of each.  Returns false when the matcher has no batched device pass (the lanes / sequential path is used).
-  virtual bool TryBasesOnLane(s4g_ctx* lane, const std::vector<SpeculativeBase*>& bases) const;
+  /// batched of each.  Returns false when the matcher has no batched device pass (the lanes / per-base chain is used).
+  virtual bool TryBasesOnLane(s4g_ctx* lane, const std::vector<SelectedBase*>& bases) const;
   mutable std::vector<s4g_ctx*> lanes_;  ///< extra device contexts (lane 0 is gpu_), same clouds
   bool lanes_stale_ = true;              ///< clouds changed since the lanes were loaded
-  void RunSpeculation();                 ///< runs the selected bases of spec_ concurrently
+  void SelectBase(SelectedBase* sb);     ///< the next base in RNG order, with its distances and pair-order replay
+  void RunSpeculation();                 ///< runs the selected bases of spec_
   void DiscardSpeculation();             ///< drops unconsumed bases, restores the RNG
+  /// the rest of the reference's TryOneBase for a selected base (hpp:317-359): adoption, visitor report, return value
   template <typename Visitor>
-  bool TryOneBaseSpeculative(const Visitor& v);
+  bool ConsumeBase(SelectedBase& sb, const Visitor& v);
+  /// visitor report of a best candidate (fraction -1), then AdoptIfBetter
+  template <typename Visitor>
+  void ReportAndAdopt(const int base_ids[4], const DeviceBest& best, const Visitor& v);
 
   // ---- candidate-set sharding across the GPUs of one box (SURVEY.md section 8, row e) inside this layer
   // S4PCS_DEVICES = a count ("4": the S4PCS_DEVICE ordinal and the three after it), "all" (every device of the box from

@@ -160,94 +160,27 @@ bool Match4PCSBase::Perform_N_steps(int n, Eigen::Ref<MatrixType> transformation
   return ok || current_trial_ >= number_of_trials_;
 }
 
+// Every base goes through here: select `depth` bases ahead in RNG order (one unless lanes or batches are on and this
+// Perform_N_steps call may still try more than one base), run them, then consume the oldest.
 template <typename Visitor>
 bool Match4PCSBase::TryOneBase(const Visitor& v) {
-  if (SpecDepth() > 1 && (!spec_.empty() || spec_budget_ > 1)) return TryOneBaseSpeculative(v);
-
-  Scalar invariant1, invariant2;
-  int ids[4];
-  const std::chrono::steady_clock::time_point t_sel = std::chrono::steady_clock::now();
-  const bool selected = SelectQuadrilateral(invariant1, invariant2, ids[0], ids[1], ids[2], ids[3]);
-  const std::chrono::steady_clock::time_point t_run = std::chrono::steady_clock::now();
-  if (timings_) stats_.ms_select += std::chrono::duration<double, std::milli>(t_run - t_sel).count();
-  if (!selected) return false;
-
-  const Scalar distance1 = (base_3D_[0].pos() - base_3D_[1].pos()).norm();
-  const Scalar distance2 = (base_3D_[2].pos() - base_3D_[3].pos()).norm();
-  const Scalar normal_angle1 = (base_3D_[0].normal() - base_3D_[1].normal()).norm();
-  const Scalar normal_angle2 = (base_3D_[2].normal() - base_3D_[3].normal()).norm();
-
-  // fused device pass: pairs x2 -> quads -> rigid fit -> Verify never leave HBM
-  DeviceBest best;
-  BaseOrder order;
-  PrepareBaseOrder(distance1, distance2, &order);
-  if (TryBaseOnDevice(invariant1, invariant2, distance1, distance2, normal_angle1, normal_angle2, ids, &best)) {
-    if (timings_) stats_.ms_passes += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_run).count();
-    AccountBase(best);
-    if (best.any) {
-      const Scalar lcp = Scalar(best.count) / Scalar(best.n_q);
-      if (lcp > best_LCP_) ResolveTies(gpu_, order, ids, &best);
-      if (!std::is_same<Visitor, DummyTransformVisitor>::value) {
-        MatrixType T = best.T;
-        if (v.needsGlobalTransformation()) T = GlobalTransform(T, best.centroid1, best.centroid2);
-        v(-1, lcp, T);
-      }
-      AdoptIfBetter(ids, best);
-    }
-    // reference hpp:335-347: a base without pairs or without congruent quads returns false (the loop goes on even when
-    // best_LCP_ already exceeds the threshold); only TryCongruentSet returns the threshold test
-    if (best.n_pairs[0] == 0 || best.n_pairs[1] == 0 || best.n_quads == 0) return false;
-    return best_LCP_ > options_.getTerminateThreshold();
-  }
-
-  // generic path through the three virtual stages (subclasses that only implement those)
-  std::vector<std::pair<int, int>> pairs1, pairs2;
-  std::vector<Quadrilateral> congruent_quads;
-  ExtractPairs(distance1, normal_angle1, distance_factor * options_.delta, 0, 1, &pairs1);
-  ExtractPairs(distance2, normal_angle2, distance_factor * options_.delta, 2, 3, &pairs2);
-  if (pairs1.size() == 0 || pairs2.size() == 0) return false;
-  if (!FindCongruentQuadrilaterals(invariant1, invariant2, distance_factor * options_.delta,
-                                   distance_factor * options_.delta, pairs1, pairs2, &congruent_quads))
-    return false;
-  size_t nb = 0;
-  return TryCongruentSet(ids[0], ids[1], ids[2], ids[3], congruent_quads, v, nb);
-}
-
-// Row f1: the next min(lanes, budget) bases are selected in RNG order and run concurrently (one
-// lane each); this call consumes the oldest one exactly like the sequential TryOneBase above.
-template <typename Visitor>
-bool Match4PCSBase::TryOneBaseSpeculative(const Visitor& v) {
   if (spec_.empty()) {
-    rng_consumed_ = randomGenerator_;  // nothing of this batch consumed yet: a discard restores this state
+    const int depth = SpecDepth() > 1 && spec_budget_ > 1 ? std::min(spec_budget_, NextDepth()) : 1;
+    rng_consumed_ = randomGenerator_;  // nothing of these bases consumed yet: a discard restores this state
     SnapshotBaseOrder(&order_consumed_);
-    const int ahead = std::min(spec_budget_, NextDepth());
-    for (int k = 0; k < ahead; ++k) {
-      spec_.emplace_back();
-      SpeculativeBase& sb = spec_.back();
-      const std::chrono::steady_clock::time_point t_sel = std::chrono::steady_clock::now();
-      sb.selected = SelectQuadrilateral(sb.invariant1, sb.invariant2, sb.ids[0], sb.ids[1], sb.ids[2], sb.ids[3]);
-      if (timings_) stats_.ms_select += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_sel).count();
-      if (sb.selected) {
-        sb.distance1 = (base_3D_[0].pos() - base_3D_[1].pos()).norm();
-        sb.distance2 = (base_3D_[2].pos() - base_3D_[3].pos()).norm();
-        sb.normal_angle1 = (base_3D_[0].normal() - base_3D_[1].normal()).norm();
-        sb.normal_angle2 = (base_3D_[2].normal() - base_3D_[3].normal()).norm();
-        sb.base3d = base_3D_;
-        PrepareBaseOrder(sb.distance1, sb.distance2, &sb.order);
-      }
-      sb.rng_after = randomGenerator_;
-    }
+    spec_.resize(size_t(depth));
+    for (SelectedBase& sb : spec_) SelectBase(&sb);
     try {
       const std::chrono::steady_clock::time_point t_run = std::chrono::steady_clock::now();
       RunSpeculation();
       if (timings_) stats_.ms_passes += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_run).count();
-    } catch (...) {  // lane set-up failed: leave the matcher as if no base had been selected
+    } catch (...) {  // device / lane set-up failed: leave the matcher as if no base had been selected
       DiscardSpeculation();
       throw;
     }
   }
 
-  SpeculativeBase sb = std::move(spec_.front());
+  SelectedBase sb = std::move(spec_.front());
   spec_.pop_front();
   rng_consumed_ = sb.rng_after;
   if (sb.order.valid) order_consumed_ = sb.order;
@@ -257,41 +190,49 @@ bool Match4PCSBase::TryOneBaseSpeculative(const Visitor& v) {
     DiscardSpeculation();
     std::rethrow_exception(sb.error);
   }
-  if (sb.handled) {
-    AccountBase(sb.best);
-    if (sb.best.any) {
-      const Scalar lcp = Scalar(sb.best.count) / Scalar(sb.best.n_q);
-      if (lcp > best_LCP_) {
-        if (sb.batched && sb.order.valid) {  // the tie resolution works on the base's RESIDENT quads: run this one base again
-          DeviceBest again;                  // on the primary context (same result; only for a base about to be adopted)
-          TryBaseOnLane(gpu_, sb.base3d, sb.invariant1, sb.invariant2, sb.distance1, sb.distance2, sb.normal_angle1,
-                        sb.normal_angle2, sb.ids, &again);
-          sb.lane = gpu_;
-        }
-        ResolveTies(sb.lane, sb.order, sb.ids, &sb.best);
-      }
-      if (!std::is_same<Visitor, DummyTransformVisitor>::value) {
-        MatrixType T = sb.best.T;
-        if (v.needsGlobalTransformation()) T = GlobalTransform(T, sb.best.centroid1, sb.best.centroid2);
-        v(-1, lcp, T);
-      }
-      AdoptIfBetter(sb.ids, sb.best);
-    }
-    if (sb.best.n_pairs[0] == 0 || sb.best.n_pairs[1] == 0 || sb.best.n_quads == 0) return false;   // (as above)
-    return best_LCP_ > options_.getTerminateThreshold();
+  return ConsumeBase(sb, v);
+}
+
+template <typename Visitor>
+bool Match4PCSBase::ConsumeBase(SelectedBase& sb, const Visitor& v) {
+  if (!sb.handled) {  // subclass without a fused device pass (or S4PCS_FUSED=0): the three virtual stages
+    std::vector<std::pair<int, int>> pairs1, pairs2;
+    std::vector<Quadrilateral> congruent_quads;
+    ExtractPairs(sb.distance1, sb.normal_angle1, distance_factor * options_.delta, 0, 1, &pairs1);
+    ExtractPairs(sb.distance2, sb.normal_angle2, distance_factor * options_.delta, 2, 3, &pairs2);
+    if (pairs1.size() == 0 || pairs2.size() == 0) return false;
+    if (!FindCongruentQuadrilaterals(sb.invariant1, sb.invariant2, distance_factor * options_.delta,
+                                     distance_factor * options_.delta, pairs1, pairs2, &congruent_quads))
+      return false;
+    size_t nb = 0;
+    return TryCongruentSet(sb.ids[0], sb.ids[1], sb.ids[2], sb.ids[3], congruent_quads, v, nb);
   }
 
-  // subclass without a fused device pass: the three virtual stages, sequentially
-  std::vector<std::pair<int, int>> pairs1, pairs2;
-  std::vector<Quadrilateral> congruent_quads;
-  ExtractPairs(sb.distance1, sb.normal_angle1, distance_factor * options_.delta, 0, 1, &pairs1);
-  ExtractPairs(sb.distance2, sb.normal_angle2, distance_factor * options_.delta, 2, 3, &pairs2);
-  if (pairs1.size() == 0 || pairs2.size() == 0) return false;
-  if (!FindCongruentQuadrilaterals(sb.invariant1, sb.invariant2, distance_factor * options_.delta,
-                                   distance_factor * options_.delta, pairs1, pairs2, &congruent_quads))
-    return false;
-  size_t nb = 0;
-  return TryCongruentSet(sb.ids[0], sb.ids[1], sb.ids[2], sb.ids[3], congruent_quads, v, nb);
+  AccountBase(sb.best);
+  if (sb.best.any && Scalar(sb.best.count) / Scalar(sb.best.n_q) > best_LCP_) {
+    if (sb.batched && sb.order.valid) {  // the tie resolution works on the base's RESIDENT quads: run this one base again
+      DeviceBest again;                  // on the primary context (same result; only for a base about to be adopted)
+      TryBaseOnLane(gpu_, sb, &again);
+      sb.lane = gpu_;
+    }
+    ResolveTies(sb.lane, sb.order, sb.ids, &sb.best);
+  }
+  ReportAndAdopt(sb.ids, sb.best, v);
+  // reference hpp:335-347: a base without pairs or without congruent quads returns false (the loop goes on even when
+  // best_LCP_ already exceeds the threshold); only TryCongruentSet returns the threshold test
+  if (sb.best.n_pairs[0] == 0 || sb.best.n_pairs[1] == 0 || sb.best.n_quads == 0) return false;
+  return best_LCP_ > options_.getTerminateThreshold();
+}
+
+template <typename Visitor>
+void Match4PCSBase::ReportAndAdopt(const int base_ids[4], const DeviceBest& best, const Visitor& v) {
+  if (!best.any) return;
+  if (!std::is_same<Visitor, DummyTransformVisitor>::value) {
+    MatrixType T = best.T;
+    if (v.needsGlobalTransformation()) T = GlobalTransform(T, best.centroid1, best.centroid2);
+    v(-1, Scalar(best.count) / Scalar(best.n_q), T);
+  }
+  AdoptIfBetter(base_ids, best);
 }
 
 template <typename Visitor>
@@ -302,17 +243,9 @@ bool Match4PCSBase::TryCongruentSet(int base_id1, int base_id2, int base_id3, in
   DeviceBest best;
   DeviceTryCongruentSet(ids, congruent_quads, &best);
   nbCongruent = best.n_gate_pass;
-  if (best.any) {
-    const Scalar lcp = Scalar(best.count) / Scalar(best.n_q);
-    // The reference reports every verified candidate; the batched device pass reports the
-    // best candidate of the set (callers in the reference tree ignore fraction < 0 reports).
-    if (!std::is_same<Visitor, DummyTransformVisitor>::value) {
-      MatrixType T = best.T;
-      if (v.needsGlobalTransformation()) T = GlobalTransform(T, best.centroid1, best.centroid2);
-      v(-1, lcp, T);
-    }
-    AdoptIfBetter(ids, best);
-  }
+  // The reference reports every verified candidate; the batched device pass reports the
+  // best candidate of the set (callers in the reference tree ignore fraction < 0 reports).
+  ReportAndAdopt(ids, best, v);
   return best_LCP_ > options_.getTerminateThreshold();
 }
 

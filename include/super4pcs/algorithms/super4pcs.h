@@ -40,13 +40,8 @@ class MatchSuper4PCS : public Match4PCSBase {
 
   void Initialize(const std::vector<Point3D>& P, const std::vector<Point3D>& Q) override;
 
-  bool TryBaseOnDevice(Scalar invariant1, Scalar invariant2, Scalar distance1, Scalar distance2,
-                       Scalar normal_angle1, Scalar normal_angle2, const int base_ids[4],
-                       DeviceBest* out) override;
-  bool TryBaseOnLane(s4g_ctx* lane, const std::vector<Point3D>& base3d, Scalar invariant1, Scalar invariant2,
-                     Scalar distance1, Scalar distance2, Scalar normal_angle1, Scalar normal_angle2,
-                     const int base_ids[4], DeviceBest* out) const override;
-  bool TryBasesOnLane(s4g_ctx* lane, const std::vector<SpeculativeBase*>& bases) const override;
+  bool TryBaseOnLane(s4g_ctx* lane, const SelectedBase& base, DeviceBest* out) const override;
+  bool TryBasesOnLane(s4g_ctx* lane, const std::vector<SelectedBase*>& bases) const override;
 
   // S4PCS_EXACT_ORDER=1: candidates in the reference's order, so that even candidates with equal inlier counts are
   // resolved like the reference does (cpp/pair_order.h; DESIGN.md section 4)
