@@ -378,6 +378,21 @@ Match4PCSBase::Scalar Match4PCSBase::Verify(const Eigen::Ref<const MatrixType>& 
   return Scalar(count) / Scalar(sampled_Q_3D_.size());
 }
 
+void Match4PCSBase::getCorrespondences(std::vector<int>* nearest, std::vector<float>* sq_dist) const {
+  // gpu_ holds the clouds init() uploaded; transform_ is the centred transform behind best_LCP_ (the identity when
+  // nothing beat it).  No context or no sampled cloud: ComputeTransformation has not run, or returned kLargeNumber.
+  if (gpu_ == nullptr || sampled_P_3D_.empty() || sampled_Q_3D_.empty())
+    throw std::runtime_error("super4pcs-b200: getCorrespondences: no registration has run on this matcher");
+  if (nearest == nullptr) throw std::invalid_argument("super4pcs-b200: getCorrespondences: nearest is null");
+  const MatrixType T = transform_;
+  nearest->resize(sampled_Q_3D_.size());
+  static_assert(sizeof(int) == sizeof(int32_t), "index type");
+  if (sq_dist) sq_dist->resize(sampled_Q_3D_.size());
+  if (s4g_verify_nearest(gpu_, T.data(), 1, reinterpret_cast<int32_t*>(nearest->data()), sq_dist ? sq_dist->data() : nullptr,
+                         nullptr) != S4G_OK)
+    ThrowLaneError(gpu_, "s4g_verify_nearest");
+}
+
 bool Match4PCSBase::TryBaseOnLane(s4g_ctx*, const SelectedBase&, DeviceBest*) const { return false; }
 
 bool Match4PCSBase::TryBasesOnLane(s4g_ctx*, const std::vector<SelectedBase*>&) const { return false; }

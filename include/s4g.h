@@ -94,6 +94,22 @@ int s4g_get_grid_stats(s4g_ctx* ctx, double* out6);
 int s4g_verify(s4g_ctx* ctx, const float* T_colmajor, int K, uint32_t* counts);
 int s4g_verify_dev(s4g_ctx* ctx, const float* d_T_colmajor, int K, uint32_t* d_counts);
 int s4g_verify_probe_stats(s4g_ctx* ctx, const float* T_colmajor, int K, uint64_t* out5);
+/* The neighbour Verify looks up and drops: for every sampled-Q point i (the order of s4g_set_cloud_q) and each of K
+ * transforms, the sampled-P point nearest to T q_i within delta (reference match4pcsBase.cc:531-536, the query of
+ * KdTree::doQueryRestrictedClosestIndex, accelerators/kdtree.h:388-453).  T q and d^2 = dx^2 + (dy^2 + dz^2) use the
+ * arithmetic of s4g_verify (fp32, reference operation order, no FMA; kdtree.h:417-418).
+ *   index[k * n_Q + i]   = j, the position in the array passed to s4g_set_cloud_p (= in sampled_P_3D_, the order
+ *                          initKdTree adds the points in, match4pcsBase.cc:353-363) with the smallest d^2 <= delta^2;
+ *                          -1 when there is none
+ *   sq_dist[k * n_Q + i] = that d^2, bit for bit; +inf when index = -1 (sq_dist may be NULL)
+ *   counts[k]            = #{i : index[k * n_Q + i] >= 0} = s4g_verify's count for the same T (counts may be NULL)
+ * Tie rule -- the one deliberate difference from the reference: among points of equal d^2 the SMALLEST j wins.  The
+ * kd-tree keeps the last one its traversal visits (sqdist <= cl_dist, kdtree.h:417), an artefact of the tree's shape.
+ * So sq_dist equals the reference's wherever it finds a neighbour, and index equals it wherever the minimum is unique.
+ * _dev: device buffers (d_index / d_sq_dist: K x n_Q), enqueued on the context's stream, nothing synchronised.       */
+int s4g_verify_nearest(s4g_ctx* ctx, const float* T_colmajor, int K, int32_t* index, float* sq_dist, uint32_t* counts);
+int s4g_verify_nearest_dev(s4g_ctx* ctx, const float* d_T_colmajor, int K, int32_t* d_index, float* d_sq_dist,
+                           uint32_t* d_counts);
 /* Verify + the first-maximum rule of TryCongruentSet (algorithms/match4pcsBase.hpp:467-484) in one stream-ordered chain:
  * counts as s4g_verify*, then key = max_k (counts[k] << 32) | (0xFFFFFFFF - index[k])  (index = the candidates' positions
  * in the caller's whole list; NULL = k), then -- when a communicator is attached, s4g_comm_* below -- the maximum over all

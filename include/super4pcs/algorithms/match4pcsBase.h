@@ -61,6 +61,12 @@ class Match4PCSBase {
   /// centred sampled clouds used by the registration
   inline const std::vector<Point3D>& getFirstSampled() const { return sampled_P_3D_; }
   inline const std::vector<Point3D>& getSecondSampled() const { return sampled_Q_3D_; }
+  /// After ComputeTransformation: for every point of getSecondSampled(), the index into getFirstSampled() of its
+  /// nearest point within options.delta under the transform that was found (-1: none) -- the neighbour the
+  /// reference's Verify looks up; the number of entries >= 0 is best LCP x |sampled Q|.  sq_dist: optional.
+  /// Equal distances resolve to the smallest index (s4g_verify_nearest).  Throws std::runtime_error when no
+  /// registration has run on this object, or it ended early (kLargeNumber), or the device call fails.
+  void getCorrespondences(std::vector<int>* nearest, std::vector<float>* sq_dist = nullptr) const;
 
   /// Approximates the best LCP between P and Q and the rigid motion realising it; on success
   /// Q is replaced by the transformed input.  Returns the LCP in [0,1], or kLargeNumber when Q is

@@ -3,9 +3,11 @@
   cfg1  50K-pt pair, 40 % overlap, delta=0.01: ExtractPairs d=1.0 (ordered pairs/s), one whole base
         (pairs x2 -> quads -> TryCongruentSet) at |sampled_Q| = 3000 / 10000, Verify at 50K x 50K
   cfg3  200K-pt pair + noise + outliers, normals on (max_normal_difference = 30 deg), n = 10000
+  cfg2  1M x 1M pair, delta=0.003: the nearest P point within delta of every query (s4g_verify_nearest_dev), ms per
+        transform for a near-ground-truth and a wrong transform, CUDA events, with the card's name and power limit
   cfg4  10M-pt pair: grid build (points/s) and the counting-only shell query at eps = 2e-4
 
-usage: python scripts/stage_bench.py [cfg1] [cfg3] [cfg4]   -> one JSON line per figure
+usage: python scripts/stage_bench.py [cfg1] [cfg2] [cfg3] [cfg4]   -> one JSON line per figure
 """
 import json
 import os
@@ -98,6 +100,46 @@ def cfg1():
                 out(cfg="cfg1", stage="base", sample_size=ns, base=b, **whole_base(ctx, P, rng, delta))
 
 
+def cfg2(reps=20):
+    import torch
+    n, delta = 1_000_000, 0.003
+    d = synth.make_pair(n, 0.3, seed=42)
+    P, cp = synth.center(d["P"])
+    Q, cq = synth.center(d["Q"])
+    M = synth.candidate_transforms(2, delta, seed=7, n_near=1, centroid_p=cp, centroid_q=cq)   # near-GT, then a random one
+    T = np.ascontiguousarray(M.transpose(0, 2, 1)).reshape(-1, 16)
+    stream = torch.cuda.Stream()            # an explicit stream: handle 0 would mean the context's own stream
+    with Context(0) as ctx, torch.cuda.stream(stream):
+        ctx.set_cloud_p(P, delta)
+        ctx.set_cloud_q(Q)
+        ctx.set_stream(stream.cuda_stream)
+        gs = ctx.grid_stats()
+        counts = ctx.verify(T)
+        idx = torch.empty(n, dtype=torch.int32, device="cuda")
+        sq = torch.empty(n, dtype=torch.float32, device="cuda")
+        cnt = torch.empty(1, dtype=torch.int32, device="cuda")
+        for k, which in enumerate(("near_gt", "wrong")):
+            dT = torch.from_numpy(T[k:k + 1].copy()).cuda()
+            call = lambda: ctx.verify_nearest_dev(dT.data_ptr(), 1, idx.data_ptr(), sq.data_ptr(), cnt.data_ptr())  # noqa: E731
+            call()
+            stream.synchronize()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(stream)
+            for _ in range(reps):
+                call()
+            e1.record(stream)
+            e1.synchronize()
+            ms = e0.elapsed_time(e1) / reps
+            hits = int(cnt.item())
+            assert hits == int(counts[k]), "nearest count differs from Verify's"
+            # bytes model: every query read (16 B) and its index + sq_dist written (8 B), plus the grid and the sorted P
+            # (the resident bytes of the grid statistics) read once -- an upper-end model for a wrong transform, whose
+            # queries mostly land outside the occupied cells and read little of the grid
+            out(cfg="cfg2", stage="verify_nearest", transform=which, n_p=n, n_q=n, delta=delta, inliers=hits,
+                ms_per_transform=ms, queries_per_s=n / (ms * 1e-3), roofline=roofline(n * 24.0 + gs["resident_bytes"], ms),
+                device=bench.device_info(0, 0))
+
+
 def cfg3():
     n, delta = 200_000, 0.01
     d = synth.make_pair(n, 0.4, seed=43, noise_sigma=0.005, outlier_frac=0.2, with_normals=True)
@@ -132,4 +174,4 @@ def cfg4():
 if __name__ == "__main__":
     which = sys.argv[1:] or ["cfg1"]
     for w in which:
-        {"cfg1": cfg1, "cfg3": cfg3, "cfg4": cfg4}[w]()
+        {"cfg1": cfg1, "cfg2": cfg2, "cfg3": cfg3, "cfg4": cfg4}[w]()

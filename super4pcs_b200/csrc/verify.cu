@@ -162,6 +162,21 @@ __device__ __forceinline__ void exact_tq(const float* __restrict__ m, float4 q, 
   tz = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[8], q.x), __fmul_rn(m[9], q.y)), __fmul_rn(m[10], q.z)), m[11]);
 }
 
+// Origin (x0,y0,z0) of the 2x2x2 cell block around t = T q that holds every P point within delta of t (conservative, see
+// the header).  false: t is so far outside the grid that no P point is within delta (x0.. are then left unset).
+__device__ __forceinline__ bool block_origin(const GridDev& g, float tx, float ty, float tz, int& x0, int& y0, int& z0) {
+  const float ux = __fsub_rn(__fmul_rn(__fsub_rn(tx, g.ox), g.inv_h), 0.5f);
+  const float uy = __fsub_rn(__fmul_rn(__fsub_rn(ty, g.oy), g.inv_h), 0.5f);
+  const float uz = __fsub_rn(__fmul_rn(__fsub_rn(tz, g.oz), g.inv_h), 0.5f);
+  const bool in = ux >= -1.f && uy >= -1.f && uz >= -1.f && ux < (float)g.nx && uy < (float)g.ny && uz < (float)g.nz;
+  if (in) {
+    x0 = __float2int_rd(ux);
+    y0 = __float2int_rd(uy);
+    z0 = __float2int_rd(uz);
+  }
+  return in;
+}
+
 // voxel coordinates of the query under one candidate.  Fast path: FMA chain of the voxel-space matrix (selection only,
 // its rounding is covered by the field's margin for candidates that passed the bound check).  Robust path: from the
 // reference-order T q (accurate to 1e-3 voxel for any T).
@@ -439,14 +454,9 @@ k_verify(GridDev g, const float4* __restrict__ Q, const float4* __restrict__ til
           const float4 qq = __ldg(&Q[qbase + (long long)(e & 1023u)]);
           float tx, ty, tz;
           exact_tq(&sT[c * 12], qq, tx, ty, tz);
-          // origin of the 2x2x2 cell block around t (conservative, see the header)
-          const float ux = __fsub_rn(__fmul_rn(__fsub_rn(tx, g.ox), g.inv_h), 0.5f);
-          const float uy = __fsub_rn(__fmul_rn(__fsub_rn(ty, g.oy), g.inv_h), 0.5f);
-          const float uz = __fsub_rn(__fmul_rn(__fsub_rn(tz, g.oz), g.inv_h), 0.5f);
-          const bool in = ux >= -1.f && uy >= -1.f && uz >= -1.f && ux < (float)g.nx && uy < (float)g.ny && uz < (float)g.nz;
           bool found = false;
-          if (in) {
-            const int x0 = __float2int_rd(ux), y0 = __float2int_rd(uy), z0 = __float2int_rd(uz);
+          int x0, y0, z0;
+          if (block_origin(g, tx, ty, tz, x0, y0, z0)) {
             uint32_t nib = block_rows(g, x0, y0, z0);
             if (kStats) st.bitmap += 2;
 #pragma unroll 1
@@ -481,6 +491,83 @@ k_verify(GridDev g, const float4* __restrict__ Q, const float4* __restrict__ til
     atomicAdd(&stats[3], st.bitmap);
     atomicAdd(&stats[4], st.culled);   // (32-query sub-tile, candidate) pairs culled (lane 0 of every warp counted them)
   }
+}
+
+// ---- nearest P point within delta of every query (s4g_verify_nearest).  Same decision arithmetic as the exact test of
+// k_verify -- exact T q, block_origin, block_rows -- but every point of the block's non-empty rows is scanned (no first
+// hit) and the lexicographic minimum of (d^2, original P index) is kept, so the winner does not depend on the sort order
+// of the grid.  best_d2 starts at delta^2 and best_j at INT_MAX: a point is taken iff d^2 <= delta^2 and it beats the best
+// so far, exactly the hit test of k_verify; NaN distances compare false and are never taken.
+__device__ __forceinline__ void nearest_run(const GridDev& g, uint32_t s, uint32_t e, float tx, float ty, float tz,
+                                            float& best_d2, int& best_j) {
+  for (uint32_t k = s; k < e; ++k) {
+    const float4 p = __ldg(&g.pts[k]);
+    const float dx = __fsub_rn(tx, p.x), dy = __fsub_rn(ty, p.y), dz = __fsub_rn(tz, p.z);
+    const float d2 = __fadd_rn(__fmul_rn(dx, dx), __fadd_rn(__fmul_rn(dy, dy), __fmul_rn(dz, dz)));
+    const int j = __float_as_int(p.w);
+    if (d2 < best_d2 || (d2 == best_d2 && j < best_j)) {
+      best_d2 = d2;
+      best_j = j;
+    }
+  }
+}
+
+// every P point of row r (cells (x0..x0+1, y0 + (r&1), z0 + (r>>1))) of the block with origin (x0,y0,z0); the caller
+// guarantees -1 <= x0 <= nx-1 (same for y, z).  The two cells are one run when they share a brick, else one run each.
+__device__ __forceinline__ void nearest_row(const GridDev& g, int x0, int y0, int z0, int r, float tx, float ty, float tz,
+                                            float& best_d2, int& best_j) {
+  const BrickShape b = brick_shape(g);
+  const int cz = z0 + (r >> 1), cy = y0 + (r & 1);
+  if (cz < 0 || cz >= g.nz || cy < 0 || cy >= g.ny) return;
+  const int xa = max(x0, 0), xb = min(x0 + 1, g.nx - 1);
+  const bool same_brick = brick_in_row(b, 0, xa) == brick_in_row(b, 0, xb);
+  const int rowb = brick_row(g, b, cy, cz);
+  const uint32_t rowl = cell_row(b, cy, cz);
+  const int ra = __ldg(&g.top[brick_in_row(b, rowb, xa)]);
+  if (ra >= 0) {
+    const uint32_t idx = cell_in_row(b, ra, rowl, xa);
+    const uint32_t e = __ldg(&g.cellStart[idx + (same_brick ? (uint32_t)(xb - xa) : 0u) + 1u]);
+    nearest_run(g, __ldg(&g.cellStart[idx]), e, tx, ty, tz, best_d2, best_j);
+  }
+  if (!same_brick) {
+    const int rb = __ldg(&g.top[brick_in_row(b, rowb, xb)]);
+    if (rb >= 0) {
+      const uint32_t idx = cell_in_row(b, rb, rowl, xb);
+      nearest_run(g, __ldg(&g.cellStart[idx]), __ldg(&g.cellStart[idx + 1u]), tx, ty, tz, best_d2, best_j);
+    }
+  }
+}
+
+// One thread per query (Morton order, so that the block look-ups of a warp stay local), blockIdx.y = transform k0 + y.
+// index / sq_dist rows are written at the query's original position; counts[k] gets one atomic per CTA.
+__global__ void __launch_bounds__(kThreads)
+k_verify_nearest(GridDev g, const float4* __restrict__ Q, int nQ, const VerifyCand* __restrict__ recs, int k0, float sq_eps,
+                 int32_t* __restrict__ index, float* __restrict__ sq_dist, uint32_t* __restrict__ counts) {
+  const int k = k0 + (int)blockIdx.y;
+  const long long qi = (long long)blockIdx.x * kThreads + threadIdx.x;
+  bool found = false;
+  if (qi < nQ) {
+    const float4 q = __ldg(&Q[qi]);
+    float tx, ty, tz;
+    exact_tq(recs[k].T, q, tx, ty, tz);
+    float best_d2 = sq_eps;
+    int best_j = 0x7fffffff;
+    int x0, y0, z0;
+    if (block_origin(g, tx, ty, tz, x0, y0, z0)) {
+      uint32_t nib = block_rows(g, x0, y0, z0);
+      while (nib) {
+        const int r = __ffs(nib) - 1;
+        nib &= nib - 1u;
+        nearest_row(g, x0, y0, z0, r, tx, ty, tz, best_d2, best_j);
+      }
+    }
+    found = best_j != 0x7fffffff;
+    const size_t at = (size_t)k * (size_t)nQ + (size_t)__float_as_int(q.w);
+    index[at] = found ? best_j : -1;
+    if (sq_dist != nullptr) sq_dist[at] = found ? best_d2 : __int_as_float(0x7f800000);
+  }
+  const int n = __syncthreads_count(found);
+  if (counts != nullptr && threadIdx.x == 0 && n > 0) atomicAdd(&counts[k], (uint32_t)n);
 }
 
 // column-major 4x4 (16 floats) -> the candidate's record (one thread per candidate)
@@ -687,5 +774,52 @@ extern "C" int s4g_verify_probe_stats(s4g_ctx* ctx, const float* T, int K, uint6
   S4G_CUDA(cudaMemcpyAsync(h, ctx->dMisc.p, 40, cudaMemcpyDeviceToHost, st));
   S4G_CUDA(cudaStreamSynchronize(st));
   for (int i = 0; i < 5; ++i) out5[i] = h[i];
+  return S4G_OK;
+}
+
+extern "C" int s4g_verify_nearest_dev(s4g_ctx* ctx, const float* d_T, int K, int32_t* d_index, float* d_sq_dist,
+                                      uint32_t* d_counts) {
+  if (!ctx) return S4G_ERR_ARG;
+  if (K < 0 || (K > 0 && (!d_T || !d_index))) { ctx->err = "s4g_verify_nearest_dev: bad arguments"; return S4G_ERR_ARG; }
+  S4G_TRY(check_ready(ctx, "s4g_verify_nearest_dev"));
+  if (K == 0) return S4G_OK;
+  S4G_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  S4G_TRY(s4g_reserve(ctx, ctx->dVrec, (size_t)K * sizeof(VerifyCand)));
+  k_pack_rec<<<(K + 127) / 128, 128, 0, st>>>(d_T, K, s4g_verify_rec_args(ctx), ctx->dVrec.as<VerifyCand>());
+  ctx->launches++;
+  if (d_counts != nullptr) S4G_CUDA(cudaMemsetAsync(d_counts, 0, (size_t)K * sizeof(uint32_t), st));
+  const unsigned nblk = (unsigned)((ctx->nQ + kThreads - 1) / kThreads);
+  constexpr int kMaxY = 65535;   // gridDim.y limit: slabs of transforms beyond it
+  for (int k0 = 0; k0 < K; k0 += kMaxY) {
+    const dim3 grid(nblk, (unsigned)std::min(kMaxY, K - k0));
+    k_verify_nearest<<<grid, kThreads, 0, st>>>(ctx->grid, ctx->dQmorton.as<float4>(), ctx->nQ, ctx->dVrec.as<VerifyCand>(),
+                                                k0, ctx->delta * ctx->delta, d_index, d_sq_dist, d_counts);
+    ctx->launches++;
+  }
+  S4G_CUDA(cudaGetLastError());
+  return S4G_OK;
+}
+
+extern "C" int s4g_verify_nearest(s4g_ctx* ctx, const float* T, int K, int32_t* index, float* sq_dist, uint32_t* counts) {
+  if (!ctx) return S4G_ERR_ARG;
+  if (K < 0 || (K > 0 && (!T || !index))) { ctx->err = "s4g_verify_nearest: bad arguments"; return S4G_ERR_ARG; }
+  S4G_TRY(check_ready(ctx, "s4g_verify_nearest"));
+  if (K == 0) return S4G_OK;
+  S4G_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t n = (size_t)K * (size_t)ctx->nQ;
+  S4G_TRY(s4g_reserve(ctx, ctx->dScratchA, (size_t)K * 16 * sizeof(float)));
+  S4G_TRY(s4g_reserve(ctx, ctx->dScratchB, n * sizeof(int32_t)));
+  if (sq_dist != nullptr) S4G_TRY(s4g_reserve(ctx, ctx->dScratchC, n * sizeof(float)));
+  S4G_TRY(s4g_reserve(ctx, ctx->dCounts, (size_t)K * sizeof(uint32_t)));
+  S4G_CUDA(cudaMemcpyAsync(ctx->dScratchA.p, T, (size_t)K * 16 * sizeof(float), cudaMemcpyHostToDevice, st));
+  S4G_TRY(s4g_verify_nearest_dev(ctx, ctx->dScratchA.as<float>(), K, ctx->dScratchB.as<int32_t>(),
+                                 sq_dist != nullptr ? ctx->dScratchC.as<float>() : nullptr, ctx->dCounts.as<uint32_t>()));
+  S4G_CUDA(cudaMemcpyAsync(index, ctx->dScratchB.p, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  if (sq_dist != nullptr) S4G_CUDA(cudaMemcpyAsync(sq_dist, ctx->dScratchC.p, n * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if (counts != nullptr)
+    S4G_CUDA(cudaMemcpyAsync(counts, ctx->dCounts.p, (size_t)K * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  S4G_CUDA(cudaStreamSynchronize(st));
   return S4G_OK;
 }

@@ -91,6 +91,8 @@ def load_library():
         "s4g_verify": ([vp, vp, i32, vp], i32),
         "s4g_verify_dev": ([vp, vp, i32, vp], i32),
         "s4g_verify_probe_stats": ([vp, vp, i32, vp], i32),
+        "s4g_verify_nearest": ([vp, vp, i32, vp, vp, vp], i32),
+        "s4g_verify_nearest_dev": ([vp, vp, i32, vp, vp, vp], i32),
         "s4g_verify_best_dev": ([vp, vp, i32, vp, vp, vp], i32),
         "s4g_verify_best": ([vp, vp, i32, vp, vp, vp], i32),
         "s4g_comm_unique_id": ([vp], i32),
@@ -242,6 +244,22 @@ class Context:
 
     def verify_dev(self, d_T_ptr, K, d_counts_ptr):
         self._chk(self._L.s4g_verify_dev(self.h, C.c_void_p(d_T_ptr), int(K), C.c_void_p(d_counts_ptr)))
+
+    def verify_nearest(self, T_colmajor):
+        """-> (index [K, n_Q] int32, sq_dist [K, n_Q] float32, counts [K] uint32): for every sampled-Q point the sampled-P
+        point nearest to T q within delta (-1 / +inf: none; equal distances -> the smallest P index), see s4g.h"""
+        T = _c(T_colmajor).reshape(-1, 16)
+        K = len(T)
+        index, sq = np.empty((K, self.nQ), np.int32), np.empty((K, self.nQ), _f)
+        counts = np.zeros(K, np.uint32)
+        self._chk(self._L.s4g_verify_nearest(self.h, _p(T), K, _p(index), _p(sq), _p(counts)))
+        return index, sq, counts
+
+    def verify_nearest_dev(self, d_T_ptr, K, d_index_ptr, d_sq_dist_ptr=None, d_counts_ptr=None):
+        """device pointers (K x n_Q int32 / float32, K uint32; the last two may be None), stream-ordered, nothing synchronised"""
+        self._chk(self._L.s4g_verify_nearest_dev(self.h, C.c_void_p(d_T_ptr), int(K), C.c_void_p(d_index_ptr),
+                                                 C.c_void_p(d_sq_dist_ptr) if d_sq_dist_ptr else None,
+                                                 C.c_void_p(d_counts_ptr) if d_counts_ptr else None))
 
     def verify_best_dev(self, d_T_ptr, K, d_index_ptr, d_counts_ptr, d_key_ptr):
         """Verify + first-maximum key (+ the maximum over the communicator's ranks), stream-ordered, nothing synchronised"""
