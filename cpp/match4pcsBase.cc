@@ -223,9 +223,34 @@ void Match4PCSBase::UploadCloudsToAll(const std::vector<s4g_ctx*>& contexts) con
     if (e) std::rethrow_exception(e);
 }
 
-// The reference computes the mean nearest-neighbour distance of sampled P here and never uses it
-// (match4pcsBase.hpp:168-171); it consumes no random numbers, so it is not recomputed.
-Match4PCSBase::Scalar Match4PCSBase::MeanDistance() { return P_mean_distance_; }
+// match4pcsBase.cc:158-182: for every sampled-P point, its nearest other sampled-P point with d^2 <= 0.2 x P_diameter_
+// (a length passed as a squared radius, as the reference does), then the mean of those distances summed in index order.
+// gpu_ holds sampled P since init uploaded it; the query excludes the point itself (the kd-tree's currentId = i).  Equal
+// d^2 give equal norms, so the tie rule of s4g_nearest does not change the value.
+Match4PCSBase::Scalar Match4PCSBase::MeanDistance() {
+  const Scalar kDiameterFraction = 0.2;
+  int number_of_samples = 0;
+  Scalar distance = 0.0;
+  const int n = int(sampled_P_3D_.size());
+  if (n > 0) {
+    if (gpu_ == nullptr) throw std::runtime_error("super4pcs-b200: MeanDistance: no clouds on the device (call init first)");
+    std::vector<float> xyz(3 * size_t(n));
+    std::vector<int32_t> self(n), nearest(n);
+    for (int i = 0; i < n; ++i) {
+      for (int k = 0; k < 3; ++k) xyz[3 * size_t(i) + k] = sampled_P_3D_[i].pos()[k];
+      self[i] = i;
+    }
+    if (s4g_nearest(gpu_, xyz.data(), n, nullptr, P_diameter_ * kDiameterFraction, self.data(), nearest.data(), nullptr) !=
+        S4G_OK)
+      ThrowLaneError(gpu_, "s4g_nearest");
+    for (int i = 0; i < n; ++i) {
+      if (nearest[i] < 0) continue;
+      distance += (sampled_P_3D_[i].pos() - sampled_P_3D_[nearest[i]].pos()).norm();
+      number_of_samples++;
+    }
+  }
+  return distance / number_of_samples;
+}
 
 bool Match4PCSBase::SelectRandomTriangle(int& base1, int& base2, int& base3) {
   const int n = int(sampled_P_3D_.size());
@@ -391,6 +416,24 @@ void Match4PCSBase::getCorrespondences(std::vector<int>* nearest, std::vector<fl
   if (s4g_verify_nearest(gpu_, T.data(), 1, reinterpret_cast<int32_t*>(nearest->data()), sq_dist ? sq_dist->data() : nullptr,
                          nullptr) != S4G_OK)
     ThrowLaneError(gpu_, "s4g_verify_nearest");
+}
+
+void Match4PCSBase::getCorrespondences(std::vector<int>* nearest, std::vector<float>* sq_dist, Scalar max_distance) const {
+  if (gpu_ == nullptr || sampled_P_3D_.empty() || sampled_Q_3D_.empty())
+    throw std::runtime_error("super4pcs-b200: getCorrespondences: no registration has run on this matcher");
+  if (nearest == nullptr) throw std::invalid_argument("super4pcs-b200: getCorrespondences: nearest is null");
+  if (std::isnan(max_distance)) throw std::invalid_argument("super4pcs-b200: getCorrespondences: max_distance is NaN");
+  const MatrixType T = transform_;
+  const int n = int(sampled_Q_3D_.size());
+  std::vector<float> xyz(3 * size_t(n));
+  for (int i = 0; i < n; ++i)
+    for (int k = 0; k < 3; ++k) xyz[3 * size_t(i) + k] = sampled_Q_3D_[i].pos()[k];
+  nearest->resize(n);
+  if (sq_dist) sq_dist->resize(n);
+  const float sq_radius = max_distance * max_distance;   // as delta * delta (match4pcsBase.cc:522)
+  if (s4g_nearest(gpu_, xyz.data(), n, T.data(), sq_radius, nullptr, reinterpret_cast<int32_t*>(nearest->data()),
+                  sq_dist ? sq_dist->data() : nullptr) != S4G_OK)
+    ThrowLaneError(gpu_, "s4g_nearest");
 }
 
 bool Match4PCSBase::TryBaseOnLane(s4g_ctx*, const SelectedBase&, DeviceBest*) const { return false; }

@@ -110,6 +110,24 @@ int s4g_verify_probe_stats(s4g_ctx* ctx, const float* T_colmajor, int K, uint64_
 int s4g_verify_nearest(s4g_ctx* ctx, const float* T_colmajor, int K, int32_t* index, float* sq_dist, uint32_t* counts);
 int s4g_verify_nearest_dev(s4g_ctx* ctx, const float* d_T_colmajor, int K, int32_t* d_index, float* d_sq_dist,
                            uint32_t* d_counts);
+/* The restricted closest-point query of the reference's kd-tree (KdTree::doQueryRestrictedClosestIndex,
+ * accelerators/kdtree.h:388-453) on the resident sampled P, for n arbitrary query points xyz (n x 3):
+ *   index[i]   = j with the smallest d^2 = |y_i - p_j|^2 <= sq_radius and j != exclude[i]  (-1: none),
+ *                y_i = T x_i (fp32, reference order, no FMA) or x_i when T is NULL; d^2 = dx^2 + (dy^2 + dz^2) in fp32
+ *   sq_dist[i] = that d^2 bit for bit, +inf for -1 (may be NULL)
+ * j is the position in the array passed to s4g_set_cloud_p.  sq_radius is the kd-tree's RangeQuery::sqdist: any value,
+ * +inf = unbounded; NaN -> S4G_ERR_ARG.  exclude: NULL or n entries (-1 = none) -- the kd-tree's currentId.  Ties: the
+ * smallest j (as s4g_verify_nearest).  A query with a NaN coordinate finds nothing.  The kd-tree never takes a point whose
+ * d^2 equals sq_radius when its pruning test (strict <) stops first, so at sq_radius = 0 it finds nothing at all; here
+ * d^2 <= sq_radius holds exactly.  Needs s4g_set_cloud_p only (S4G_ERR_STATE before it); n == 0 is a no-op.
+ * _dev: device buffers, enqueued on the context's stream, nothing synchronised.
+ * _probe_stats: as s4g_nearest, and out2 = {P points tested, coarse blocks scanned} summed over the queries.          */
+int s4g_nearest(s4g_ctx* ctx, const float* xyz, int n, const float* T_colmajor, float sq_radius, const int32_t* exclude,
+                int32_t* index, float* sq_dist);
+int s4g_nearest_dev(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T_colmajor, float sq_radius,
+                    const int32_t* d_exclude, int32_t* d_index, float* d_sq_dist);
+int s4g_nearest_probe_stats(s4g_ctx* ctx, const float* xyz, int n, const float* T_colmajor, float sq_radius,
+                            const int32_t* exclude, int32_t* index, float* sq_dist, uint64_t* out2);
 /* Verify + the first-maximum rule of TryCongruentSet (algorithms/match4pcsBase.hpp:467-484) in one stream-ordered chain:
  * counts as s4g_verify*, then key = max_k (counts[k] << 32) | (0xFFFFFFFF - index[k])  (index = the candidates' positions
  * in the caller's whole list; NULL = k), then -- when a communicator is attached, s4g_comm_* below -- the maximum over all

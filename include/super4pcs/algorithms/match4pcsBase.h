@@ -67,6 +67,10 @@ class Match4PCSBase {
   /// Equal distances resolve to the smallest index (s4g_verify_nearest).  Throws std::runtime_error when no
   /// registration has run on this object, or it ended early (kLargeNumber), or the device call fails.
   void getCorrespondences(std::vector<int>* nearest, std::vector<float>* sq_dist = nullptr) const;
+  /// The same at any radius: the nearest point of getFirstSampled() with distance <= max_distance (squared in fp32,
+  /// as delta is; +inf: the nearest point whatever its distance) under the transform that was found (s4g_nearest).
+  /// getCorrespondences(nearest, sq_dist, options.delta) equals the two-argument form.
+  void getCorrespondences(std::vector<int>* nearest, std::vector<float>* sq_dist, Scalar max_distance) const;
 
   /// Approximates the best LCP between P and Q and the rigid motion realising it; on success
   /// Q is replaced by the transformed input.  Returns the LCP in [0,1], or kLargeNumber when Q is
@@ -81,7 +85,7 @@ class Match4PCSBase {
   int number_of_trials_;
   Scalar max_base_diameter_;
   Scalar P_diameter_;
-  Scalar P_mean_distance_;  ///< kept for layout/API; the reference computes but never uses it
+  Scalar P_mean_distance_;  ///< kept for layout/API (1.0); the reference computes it in init but never uses it
   Eigen::Matrix<Scalar, 4, 4> transform_;
   Eigen::Matrix<Scalar, 3, 1> qcentroid1_, qcentroid2_;
   int base_[4];
@@ -108,6 +112,8 @@ class Match4PCSBase {
   template <Utils::LogLevel level, typename... Args>
   inline void Log(Args... args) const { logger_.Log<level>(args...); }
 
+  /// The reference's mean distance of every sampled-P point to its nearest other sampled-P point within squared radius
+  /// 0.2 x P_diameter_ (match4pcsBase.cc:158-182), through s4g_nearest; 0 / 0 without samples.  init does not call it.
   Scalar MeanDistance();
   bool SelectRandomTriangle(int& base1, int& base2, int& base3);
   bool TryQuadrilateral(Scalar& invariant1, Scalar& invariant2, int& base1, int& base2, int& base3, int& base4);

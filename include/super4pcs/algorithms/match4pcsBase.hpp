@@ -93,7 +93,8 @@ void Match4PCSBase::init(const std::vector<Point3D>& P, const std::vector<Point3
     const Scalar l = (sampled_Q_3D_[bt].pos() - sampled_Q_3D_[at].pos()).norm();
     if (l > P_diameter_) P_diameter_ = l;
   }
-  P_mean_distance_ = MeanDistance();
+  // The reference stores MeanDistance() here (hpp:168) and never reads it; P_mean_distance_ keeps the constructor's 1.0
+  // and MeanDistance() computes the reference's value when called.
   max_base_diameter_ = P_diameter_;
 
   // RANSAC trial count for a failure probability of kSmallError

@@ -229,7 +229,7 @@ __global__ void k_mark_coarse(GridDev g, const float4* __restrict__ P, int n, ui
   float4 p = P[i];
   int3 c = cell_of(g, p.x, p.y, p.z);
   const uint32_t X = (uint32_t)(c.x >> g.cshift) + 1u, Y = (uint32_t)(c.y >> g.cshift) + 1u, Z = (uint32_t)(c.z >> g.cshift) + 1u;
-  csat[(Z * (uint32_t)(g.cny + 1) + Y) * (uint32_t)(g.cnx + 1) + X] = 1u;
+  csat[csat_slot(g, X, Y, Z)] = 1u;
 }
 
 // occupancy nibbles of the 2x2x2-cell blocks the exact test of Verify probes (GridDev::vocc): a point in cell c marks

@@ -119,6 +119,20 @@ __device__ __forceinline__ uint32_t fine_half(uint32_t slot) { return (slot & 1u
 // vocc: nibble of block origin cell slot `cell`; bit r: row (y0 + (r & 1), z0 + (r >> 1)) of the 2x2x2-cell block has points
 __device__ __forceinline__ uint32_t vocc_word(uint32_t cell) { return cell >> 3; }
 __device__ __forceinline__ uint32_t vocc_shift(uint32_t cell) { return (cell & 7u) * 4u; }
+// csat: entry of corner (X, Y, Z) = #occupied coarse blocks with x < X, y < Y, z < Z
+__device__ __forceinline__ uint32_t csat_slot(const GridDev& g, uint32_t X, uint32_t Y, uint32_t Z) {
+  return (Z * (uint32_t)(g.cny + 1) + Y) * (uint32_t)(g.cnx + 1) + X;
+}
+// number of occupied coarse blocks in the inclusive box [x0, x1] x [y0, y1] x [z0, z1] of block coordinates (8 look-ups)
+__device__ __forceinline__ uint32_t csat_count(const GridDev& g, int x0, int x1, int y0, int y1, int z0, int z1) {
+  const uint32_t* __restrict__ S = g.csat;
+  const uint32_t X0 = (uint32_t)x0, X1 = (uint32_t)x1 + 1u, Y0 = (uint32_t)y0, Y1 = (uint32_t)y1 + 1u;
+  const uint32_t Z0 = (uint32_t)z0, Z1 = (uint32_t)z1 + 1u;
+  return (__ldg(&S[csat_slot(g, X1, Y1, Z1)]) - __ldg(&S[csat_slot(g, X0, Y1, Z1)]) - __ldg(&S[csat_slot(g, X1, Y0, Z1)]) +
+          __ldg(&S[csat_slot(g, X0, Y0, Z1)])) -
+         (__ldg(&S[csat_slot(g, X1, Y1, Z0)]) - __ldg(&S[csat_slot(g, X0, Y1, Z0)]) - __ldg(&S[csat_slot(g, X1, Y0, Z0)]) +
+          __ldg(&S[csat_slot(g, X0, Y0, Z0)]));
+}
 
 // ---- warp helpers of the Morton-ordered query side
 // AABB of the warp's boxes: every lane ends with the union

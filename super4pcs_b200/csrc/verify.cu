@@ -570,6 +570,197 @@ k_verify_nearest(GridDev g, const float4* __restrict__ Q, int nQ, const VerifyCa
   if (counts != nullptr && threadIdx.x == 0 && n > 0) atomicAdd(&counts[k], (uint32_t)n);
 }
 
+// ---- nearest P point at any radius, for arbitrary query points (s4g_nearest): the restricted closest-point query of the
+// reference's kd-tree (KdTree::doQueryRestrictedClosestIndex, kdtree.h:388-453).  One thread per query: y = T x
+// (exact_tq) or x; the answer is the lexicographic minimum of (d^2, original P index) over the P points with
+// d^2 <= sq_radius and index != exclude, d^2 = dx^2 + (dy^2 + dz^2) in fp32 as in nearest_run (nearest_run_excl).
+//
+// Search.  The cell coordinates of y, u = (y - o) * inv_h, are taken in double.  The coarse blocks of GridDev::csat
+// ((2^cshift)^3 cells) form an implicit tree of boxes: the root is the whole coarse lattice, and a box splits into two
+// halves of its longest axis down to single blocks.  The thread descends it depth first with an explicit stack, nearer
+// half first: a box is dropped when its lower bound (below) exceeds the best d^2 so far or when csat says it holds no
+// point (8 look-ups); a single block left is scanned row by row -- rows whose bound exceeds the best are skipped, the
+// others are contiguous runs of the sorted points, one per brick they cross.  best_d2 starts at sq_radius, so nothing
+// beyond the radius is ever opened.  A dropped point has a d^2 strictly above the best at that time, so it could neither
+// win nor tie: the answer is the lexicographic minimum whatever the order of the search.
+// Work: every box opened either is a block that is scanned or has a child that is not empty and within the bound, so a
+// query opens at most (1 + 2 x depth) boxes per block it scans (depth <= log2 of the lattice's extents, ~30); empty
+// space costs one look-up of csat per box, whatever its size.  The blocks scanned are those within the best distance
+// found along the way: for a query near the cloud a handful; for one far outside, those near the first hit.
+//
+// Lower bound.  A point stored in cell c (on one axis) was binned by floorf(fl(fl(p - o) * inv_h)) (context.cu, cell_of;
+// never clamped, the grid has a 1.5-cell margin): two roundings of relative size 2^-24 of a value below n + 1 cells, so
+// its exact coordinate v = (p - o) * inv_h lies in (c - eps, c + 1 + eps) with eps = (max(nx, ny, nz) + 2) * 2^-21,
+// twice the rounding (1e-3 cell for 2048 cells).  For every point binned in a box of cells, |y - p| on that axis is at least
+// gap / inv_h, gap = the distance from u to [c0 - eps, c1 + 1 + eps], so L = sum gap^2 / inv_h^2 bounds the exact d^2.  The
+// d^2 the kernel computes takes five roundings of relative size 2^-24 (plus 2^-148 when it is subnormal), so it is at
+// least L (1 - 2^-20) - 2^-140; that value, from double arithmetic (relative error ~2^-50) rounded down to fp32, is the
+// bound.  A bound that is too low only costs time; this one is never above a d^2 the kernel computes.
+struct NearestQuery {
+  float tx, ty, tz;   // y
+  int excl;           // original P index never taken (-1: none)
+  double ux, uy, uz;  // cell coordinates of y
+  double eps, h2;     // binning margin of the points (cells); squared cell edge
+};
+
+struct NearestStats {
+  unsigned long long tested = 0, blocks = 0;
+};
+
+// nearest_run (same d^2, same rule) without the point of original index q.excl.  A separate copy, so that the code of
+// k_verify_nearest stays as it is.
+__device__ __forceinline__ void nearest_run_excl(const GridDev& g, uint32_t s, uint32_t e, const NearestQuery& q,
+                                                 float& best_d2, int& best_j) {
+  for (uint32_t k = s; k < e; ++k) {
+    const float4 p = __ldg(&g.pts[k]);
+    const float dx = __fsub_rn(q.tx, p.x), dy = __fsub_rn(q.ty, p.y), dz = __fsub_rn(q.tz, p.z);
+    const float d2 = __fadd_rn(__fmul_rn(dx, dx), __fadd_rn(__fmul_rn(dy, dy), __fmul_rn(dz, dz)));
+    const int j = __float_as_int(p.w);
+    if ((d2 < best_d2 || (d2 == best_d2 && j < best_j)) && j != q.excl) {
+      best_d2 = d2;
+      best_j = j;
+    }
+  }
+}
+
+// lower bound of the d^2 k_nearest computes between y and any point binned in the cells [x0, x1] x [y0, y1] x [z0, z1]
+__device__ __forceinline__ float cells_bound(const NearestQuery& q, int x0, int x1, int y0, int y1, int z0, int z1) {
+  const double gx = fmax(0.0, fmax(((double)x0 - q.eps) - q.ux, q.ux - ((double)x1 + 1.0 + q.eps)));
+  const double gy = fmax(0.0, fmax(((double)y0 - q.eps) - q.uy, q.uy - ((double)y1 + 1.0 + q.eps)));
+  const double gz = fmax(0.0, fmax(((double)z0 - q.eps) - q.uz, q.uz - ((double)z1 + 1.0 + q.eps)));
+  const double b = (gx * gx + gy * gy + gz * gz) * q.h2 * (1.0 - 0x1p-20) - 0x1p-140;
+  return b > 0.0 ? __double2float_rd(b) : 0.f;
+}
+
+// every cell row of the cell box [x0, x1] x [y0, y1] x [z0, z1] that may hold a better point: one run per brick it crosses
+template <bool kStats>
+__device__ __forceinline__ void nearest_cells(const GridDev& g, const NearestQuery& q, int x0, int x1, int y0, int y1,
+                                              int z0, int z1, float& best_d2, int& best_j, NearestStats& st) {
+  const BrickShape b = brick_shape(g);
+#pragma unroll 1
+  for (int cz = z0; cz <= z1; ++cz)
+#pragma unroll 1
+    for (int cy = y0; cy <= y1; ++cy) {
+      if (cells_bound(q, x0, x1, cy, cy, cz, cz) > best_d2) continue;
+      const int rowb = brick_row(g, b, cy, cz);
+      const uint32_t rowl = cell_row(b, cy, cz);
+#pragma unroll 1
+      for (int x = x0; x <= x1;) {
+        const int xe = min(x1, x | b.m);   // the last cell of the row inside x's brick
+        const int rank = __ldg(&g.top[brick_in_row(b, rowb, x)]);
+        if (rank >= 0) {
+          const uint32_t s = __ldg(&g.cellStart[cell_in_row(b, rank, rowl, x)]);
+          const uint32_t e = __ldg(&g.cellStart[cell_in_row(b, rank, rowl, xe) + 1u]);
+          if (kStats) st.tested += e - s;
+          nearest_run_excl(g, s, e, q, best_d2, best_j);
+        }
+        x = xe + 1;
+      }
+    }
+}
+
+// a box of coarse blocks [x0, x1] x [y0, y1] x [z0, z1], packed lo | hi << 16 per axis (the coarse lattice has < 2^16
+// blocks per axis: its table has <= 2^20 entries)
+struct BlockBox {
+  uint32_t x, y, z;
+};
+__device__ __forceinline__ int box_lo(uint32_t a) { return (int)(a & 0xFFFFu); }
+__device__ __forceinline__ int box_hi(uint32_t a) { return (int)(a >> 16); }
+__device__ __forceinline__ uint32_t box_axis(int lo, int hi) { return (uint32_t)lo | ((uint32_t)hi << 16); }
+constexpr int kNearestStack = 3 * 16 + 1;   // depth of the box tree (<= 16 halvings per axis) + 1: the stack's most entries
+
+// One thread per query, written at its own position.  T16: column-major 4x4 or nullptr; exclude: n entries or nullptr.
+// stats (kStats): [0] += P points tested, [1] += coarse blocks scanned.
+template <bool kStats>
+__global__ void __launch_bounds__(kThreads)
+k_nearest(GridDev g, const float* __restrict__ xyz, int n, const float* __restrict__ T16, float sq_radius,
+          const int32_t* __restrict__ exclude, int32_t* __restrict__ index, float* __restrict__ sq_dist,
+          unsigned long long* __restrict__ stats) {
+  const long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
+  NearestStats st;
+  if (i < n) {
+    const float4 x = make_float4(__ldg(&xyz[3 * i]), __ldg(&xyz[3 * i + 1]), __ldg(&xyz[3 * i + 2]), 0.f);
+    NearestQuery q;
+    if (T16 != nullptr) {
+      float m[12];
+#pragma unroll
+      for (int e = 0; e < 12; ++e) m[e] = __ldg(&T16[(e & 3) * 4 + (e >> 2)]);
+      exact_tq(m, x, q.tx, q.ty, q.tz);
+    } else {
+      q.tx = x.x;
+      q.ty = x.y;
+      q.tz = x.z;
+    }
+    q.excl = exclude != nullptr ? __ldg(&exclude[i]) : -1;
+    float best_d2 = sq_radius;
+    int best_j = 0x7fffffff;
+    if (!isnan(q.tx) && !isnan(q.ty) && !isnan(q.tz)) {   // (a NaN coordinate makes every d^2 NaN: nothing is taken)
+      const double ih = (double)g.inv_h;
+      q.ux = ((double)q.tx - (double)g.ox) * ih;
+      q.uy = ((double)q.ty - (double)g.oy) * ih;
+      q.uz = ((double)q.tz - (double)g.oz) * ih;
+      q.eps = (double)(max(g.nx, max(g.ny, g.nz)) + 2) * 0x1p-21;
+      q.h2 = 1.0 / (ih * ih);
+      const int cs = g.cshift, mx = g.nx - 1, my = g.ny - 1, mz = g.nz - 1;
+      BlockBox stack[kNearestStack];
+      int top = 0;
+      stack[top++] = BlockBox{box_axis(0, g.cnx - 1), box_axis(0, g.cny - 1), box_axis(0, g.cnz - 1)};
+#pragma unroll 1
+      while (top > 0) {
+        const BlockBox b = stack[--top];
+        const int x0 = box_lo(b.x), x1 = box_hi(b.x), y0 = box_lo(b.y), y1 = box_hi(b.y), z0 = box_lo(b.z), z1 = box_hi(b.z);
+        // its cells (the last block of an axis may reach past the grid: clipped; a block wholly past it holds nothing)
+        const int cx0 = x0 << cs, cy0 = y0 << cs, cz0 = z0 << cs;
+        const int cx1 = min(((x1 + 1) << cs) - 1, mx), cy1 = min(((y1 + 1) << cs) - 1, my), cz1 = min(((z1 + 1) << cs) - 1, mz);
+        if (cx0 > cx1 || cy0 > cy1 || cz0 > cz1) continue;
+        if (cells_bound(q, cx0, cx1, cy0, cy1, cz0, cz1) > best_d2) continue;
+        if (csat_count(g, x0, x1, y0, y1, z0, z1) == 0u) continue;
+        const int ex = x1 - x0, ey = y1 - y0, ez = z1 - z0;
+        if ((ex | ey | ez) == 0) {                       // one block: its cell rows
+          if (kStats) st.blocks++;
+          nearest_cells<kStats>(g, q, cx0, cx1, cy0, cy1, cz0, cz1, best_d2, best_j, st);
+          continue;
+        }
+        // halve the longest axis; the half nearer to u is pushed last, so it is searched first
+        BlockBox lo = b, hi = b;
+        bool lo_near;
+        if (ex >= ey && ex >= ez) {
+          const int mid = (x0 + x1) >> 1;
+          lo.x = box_axis(x0, mid);
+          hi.x = box_axis(mid + 1, x1);
+          lo_near = q.ux < (double)((mid + 1) << cs);
+        } else if (ey >= ez) {
+          const int mid = (y0 + y1) >> 1;
+          lo.y = box_axis(y0, mid);
+          hi.y = box_axis(mid + 1, y1);
+          lo_near = q.uy < (double)((mid + 1) << cs);
+        } else {
+          const int mid = (z0 + z1) >> 1;
+          lo.z = box_axis(z0, mid);
+          hi.z = box_axis(mid + 1, z1);
+          lo_near = q.uz < (double)((mid + 1) << cs);
+        }
+        stack[top++] = lo_near ? hi : lo;
+        stack[top++] = lo_near ? lo : hi;
+      }
+    }
+    const bool found = best_j != 0x7fffffff;
+    index[i] = found ? best_j : -1;
+    if (sq_dist != nullptr) sq_dist[i] = found ? best_d2 : __int_as_float(0x7f800000);
+  }
+  if (kStats) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      st.tested += __shfl_down_sync(0xffffffffu, st.tested, o);
+      st.blocks += __shfl_down_sync(0xffffffffu, st.blocks, o);
+    }
+    if ((threadIdx.x & 31) == 0) {
+      atomicAdd(&stats[0], st.tested);
+      atomicAdd(&stats[1], st.blocks);
+    }
+  }
+}
+
 // column-major 4x4 (16 floats) -> the candidate's record (one thread per candidate)
 __global__ void k_pack_rec(const float* __restrict__ T16, int K, VerifyRecArgs ra, VerifyCand* __restrict__ recs) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -822,4 +1013,88 @@ extern "C" int s4g_verify_nearest(s4g_ctx* ctx, const float* T, int K, int32_t* 
     S4G_CUDA(cudaMemcpyAsync(counts, ctx->dCounts.p, (size_t)K * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   S4G_CUDA(cudaStreamSynchronize(st));
   return S4G_OK;
+}
+
+static int nearest_args(s4g_ctx* ctx, const char* who, int n, const void* xyz, float sq_radius, const void* index) {
+  if (n < 0 || (n > 0 && (!xyz || !index)) || std::isnan(sq_radius)) {
+    ctx->err = std::string(who) + ": bad arguments (n >= 0, xyz and index when n > 0, sq_radius not NaN)";
+    return S4G_ERR_ARG;
+  }
+  if (ctx->nP <= 0) {
+    ctx->err = std::string(who) + ": call s4g_set_cloud_p first";
+    return S4G_ERR_STATE;
+  }
+  return S4G_OK;
+}
+
+// enqueue k_nearest on the context's stream (stats != nullptr: the statistics variant)
+static int launch_nearest(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T, float sq_radius,
+                          const int32_t* d_exclude, int32_t* d_index, float* d_sq_dist, unsigned long long* stats) {
+  S4G_CUDA(cudaSetDevice(ctx->device));
+  const unsigned nblk = (unsigned)((n + kThreads - 1) / kThreads);
+  if (stats != nullptr)
+    k_nearest<true><<<nblk, kThreads, 0, ctx->stream>>>(ctx->grid, d_xyz, n, d_T, sq_radius, d_exclude, d_index, d_sq_dist,
+                                                        stats);
+  else
+    k_nearest<false><<<nblk, kThreads, 0, ctx->stream>>>(ctx->grid, d_xyz, n, d_T, sq_radius, d_exclude, d_index, d_sq_dist,
+                                                         nullptr);
+  ctx->launches++;
+  S4G_CUDA(cudaGetLastError());
+  return S4G_OK;
+}
+
+extern "C" int s4g_nearest_dev(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T, float sq_radius,
+                               const int32_t* d_exclude, int32_t* d_index, float* d_sq_dist) {
+  if (!ctx) return S4G_ERR_ARG;
+  S4G_TRY(nearest_args(ctx, "s4g_nearest_dev", n, d_xyz, sq_radius, d_index));
+  if (n == 0) return S4G_OK;
+  return launch_nearest(ctx, d_xyz, n, d_T, sq_radius, d_exclude, d_index, d_sq_dist, nullptr);
+}
+
+// host buffers -> the context's scratch, k_nearest, back; stats: nullptr or the two counters of the statistics variant
+static int nearest_host(s4g_ctx* ctx, const char* who, const float* xyz, int n, const float* T, float sq_radius,
+                        const int32_t* exclude, int32_t* index, float* sq_dist, uint64_t* stats) {
+  if (!ctx) return S4G_ERR_ARG;
+  S4G_TRY(nearest_args(ctx, who, n, xyz, sq_radius, index));
+  if (n == 0) return S4G_OK;
+  S4G_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t nn = (size_t)n;
+  S4G_TRY(s4g_reserve(ctx, ctx->dScratchA, nn * 3 * sizeof(float) + 16 * sizeof(float)));
+  S4G_TRY(s4g_reserve(ctx, ctx->dScratchB, nn * sizeof(int32_t)));
+  if (sq_dist != nullptr) S4G_TRY(s4g_reserve(ctx, ctx->dScratchC, nn * sizeof(float)));
+  if (exclude != nullptr) S4G_TRY(s4g_reserve(ctx, ctx->dScratchD, nn * sizeof(int32_t)));
+  if (stats != nullptr) S4G_TRY(s4g_reserve(ctx, ctx->dMisc, 256));
+  float* d_xyz = ctx->dScratchA.as<float>();
+  float* d_T = T != nullptr ? d_xyz + nn * 3 : nullptr;
+  S4G_CUDA(cudaMemcpyAsync(d_xyz, xyz, nn * 3 * sizeof(float), cudaMemcpyHostToDevice, st));
+  if (T != nullptr) S4G_CUDA(cudaMemcpyAsync(d_T, T, 16 * sizeof(float), cudaMemcpyHostToDevice, st));
+  if (exclude != nullptr)
+    S4G_CUDA(cudaMemcpyAsync(ctx->dScratchD.p, exclude, nn * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  if (stats != nullptr) S4G_CUDA(cudaMemsetAsync(ctx->dMisc.p, 0, 2 * sizeof(unsigned long long), st));
+  S4G_TRY(launch_nearest(ctx, d_xyz, n, d_T, sq_radius, exclude != nullptr ? ctx->dScratchD.as<int32_t>() : nullptr,
+                         ctx->dScratchB.as<int32_t>(), sq_dist != nullptr ? ctx->dScratchC.as<float>() : nullptr,
+                         stats != nullptr ? ctx->dMisc.as<unsigned long long>() : nullptr));
+  S4G_CUDA(cudaMemcpyAsync(index, ctx->dScratchB.p, nn * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  if (sq_dist != nullptr) S4G_CUDA(cudaMemcpyAsync(sq_dist, ctx->dScratchC.p, nn * sizeof(float), cudaMemcpyDeviceToHost, st));
+  unsigned long long h[2] = {0, 0};
+  if (stats != nullptr) S4G_CUDA(cudaMemcpyAsync(h, ctx->dMisc.p, sizeof h, cudaMemcpyDeviceToHost, st));
+  S4G_CUDA(cudaStreamSynchronize(st));
+  if (stats != nullptr) {
+    stats[0] = h[0];
+    stats[1] = h[1];
+  }
+  return S4G_OK;
+}
+
+extern "C" int s4g_nearest(s4g_ctx* ctx, const float* xyz, int n, const float* T, float sq_radius, const int32_t* exclude,
+                           int32_t* index, float* sq_dist) {
+  return nearest_host(ctx, "s4g_nearest", xyz, n, T, sq_radius, exclude, index, sq_dist, nullptr);
+}
+
+extern "C" int s4g_nearest_probe_stats(s4g_ctx* ctx, const float* xyz, int n, const float* T, float sq_radius,
+                                       const int32_t* exclude, int32_t* index, float* sq_dist, uint64_t* out2) {
+  if (ctx && !out2) { ctx->err = "s4g_nearest_probe_stats: bad arguments"; return S4G_ERR_ARG; }
+  if (out2) out2[0] = out2[1] = 0;
+  return nearest_host(ctx, "s4g_nearest_probe_stats", xyz, n, T, sq_radius, exclude, index, sq_dist, out2);
 }

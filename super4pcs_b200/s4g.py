@@ -93,6 +93,9 @@ def load_library():
         "s4g_verify_probe_stats": ([vp, vp, i32, vp], i32),
         "s4g_verify_nearest": ([vp, vp, i32, vp, vp, vp], i32),
         "s4g_verify_nearest_dev": ([vp, vp, i32, vp, vp, vp], i32),
+        "s4g_nearest": ([vp, vp, i32, vp, f32, vp, vp, vp], i32),
+        "s4g_nearest_dev": ([vp, vp, i32, vp, f32, vp, vp, vp], i32),
+        "s4g_nearest_probe_stats": ([vp, vp, i32, vp, f32, vp, vp, vp, vp], i32),
         "s4g_verify_best_dev": ([vp, vp, i32, vp, vp, vp], i32),
         "s4g_verify_best": ([vp, vp, i32, vp, vp, vp], i32),
         "s4g_comm_unique_id": ([vp], i32),
@@ -260,6 +263,30 @@ class Context:
         self._chk(self._L.s4g_verify_nearest_dev(self.h, C.c_void_p(d_T_ptr), int(K), C.c_void_p(d_index_ptr),
                                                  C.c_void_p(d_sq_dist_ptr) if d_sq_dist_ptr else None,
                                                  C.c_void_p(d_counts_ptr) if d_counts_ptr else None))
+
+    def nearest(self, xyz, sq_radius=np.inf, T=None, exclude=None, stats=False):
+        """-> (index [n] int32, sq_dist [n] float32): for every query point x the resident P point nearest to T x (x when T
+        is None) with d^2 <= sq_radius and index != exclude (-1 / +inf: none; equal distances -> the smallest P index),
+        see s4g.h.  stats=True: also {P points tested, coarse blocks scanned} summed over the queries."""
+        xyz = _c(xyz).reshape(-1, 3)
+        n = len(xyz)
+        T = None if T is None else _c(T).reshape(16)
+        exclude = None if exclude is None else _c(exclude, np.int32).reshape(n)
+        index, sq = np.empty(n, np.int32), np.empty(n, _f)
+        if not stats:
+            self._chk(self._L.s4g_nearest(self.h, _p(xyz), n, _p(T), float(sq_radius), _p(exclude), _p(index), _p(sq)))
+            return index, sq
+        out = np.zeros(2, np.uint64)
+        self._chk(self._L.s4g_nearest_probe_stats(self.h, _p(xyz), n, _p(T), float(sq_radius), _p(exclude), _p(index),
+                                                  _p(sq), _p(out)))
+        return index, sq, dict(tested=int(out[0]), blocks=int(out[1]))
+
+    def nearest_dev(self, d_xyz_ptr, n, d_index_ptr, d_sq_dist_ptr=None, sq_radius=np.inf, d_T_ptr=None, d_exclude_ptr=None):
+        """device pointers (n x 3 float32 queries, n int32 / float32 results, 16 float32 T, n int32 exclude; the last three
+        may be None), stream-ordered, nothing synchronised"""
+        v = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        self._chk(self._L.s4g_nearest_dev(self.h, v(d_xyz_ptr), int(n), v(d_T_ptr), float(sq_radius), v(d_exclude_ptr),
+                                          v(d_index_ptr), v(d_sq_dist_ptr)))
 
     def verify_best_dev(self, d_T_ptr, K, d_index_ptr, d_counts_ptr, d_key_ptr):
         """Verify + first-maximum key (+ the maximum over the communicator's ranks), stream-ordered, nothing synchronised"""
