@@ -436,6 +436,28 @@ void Match4PCSBase::getCorrespondences(std::vector<int>* nearest, std::vector<fl
     ThrowLaneError(gpu_, "s4g_nearest");
 }
 
+void Match4PCSBase::getNeighbors(std::vector<int64_t>* offsets, std::vector<int>* indices, Scalar max_distance,
+                                 std::vector<float>* sq_dist) const {
+  if (gpu_ == nullptr || sampled_P_3D_.empty() || sampled_Q_3D_.empty())
+    throw std::runtime_error("super4pcs-b200: getNeighbors: no registration has run on this matcher");
+  if (offsets == nullptr || indices == nullptr) throw std::invalid_argument("super4pcs-b200: getNeighbors: null output");
+  if (std::isnan(max_distance)) throw std::invalid_argument("super4pcs-b200: getNeighbors: max_distance is NaN");
+  const MatrixType T = transform_;
+  const int n = int(sampled_Q_3D_.size());
+  std::vector<float> xyz(3 * size_t(n));
+  for (int i = 0; i < n; ++i)
+    for (int k = 0; k < 3; ++k) xyz[3 * size_t(i) + k] = sampled_Q_3D_[i].pos()[k];
+  offsets->resize(size_t(n) + 1);
+  const float sq_radius = max_distance * max_distance;   // as getCorrespondences squares it
+  int64_t total = 0;
+  if (s4g_range(gpu_, xyz.data(), n, T.data(), sq_radius, offsets->data(), &total) != S4G_OK)
+    ThrowLaneError(gpu_, "s4g_range");
+  indices->resize(size_t(total));
+  if (sq_dist) sq_dist->resize(size_t(total));
+  if (s4g_get_range(gpu_, reinterpret_cast<int32_t*>(indices->data()), sq_dist ? sq_dist->data() : nullptr) != S4G_OK)
+    ThrowLaneError(gpu_, "s4g_get_range");
+}
+
 bool Match4PCSBase::TryBaseOnLane(s4g_ctx*, const SelectedBase&, DeviceBest*) const { return false; }
 
 bool Match4PCSBase::TryBasesOnLane(s4g_ctx*, const std::vector<SelectedBase*>&) const { return false; }

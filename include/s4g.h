@@ -128,6 +128,27 @@ int s4g_nearest_dev(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T_co
                     const int32_t* d_exclude, int32_t* d_index, float* d_sq_dist);
 int s4g_nearest_probe_stats(s4g_ctx* ctx, const float* xyz, int n, const float* T_colmajor, float sq_radius,
                             const int32_t* exclude, int32_t* index, float* sq_dist, uint64_t* out2);
+/* The range query of the reference's kd-tree (KdTree::doQueryDist / doQueryDistIndices / doQueryDistProcessIndices,
+ * accelerators/kdtree.h:231-262, body :462-514) on the resident sampled P, for n arbitrary query points xyz (n x 3):
+ * the list of query i is every j with d^2 = |y_i - p_j|^2 < sq_radius (strict, the kd-tree's point test kdtree.h:485),
+ * y_i and d^2 as in s4g_nearest, j the position in the array passed to s4g_set_cloud_p, in ascending j.  sq_radius <= 0:
+ * empty lists; +inf: every point with a finite d^2; NaN -> S4G_ERR_ARG.  A query with a NaN coordinate gets an empty
+ * list.  No index is excluded.  Output in CSR form: offsets [n + 1] (offsets[0] = 0, offsets[n] = total), list i =
+ * indices[offsets[i] .. offsets[i + 1]), sq_dist the same positions (d^2 bit for bit).  Needs s4g_set_cloud_p only
+ * (S4G_ERR_STATE before it); n == 0 writes offsets[0] = 0; a result the device cannot hold -> S4G_ERR_NOMEM.
+ *   s4g_range       writes offsets and *total, keeps the lists in the context (replacing the previous result);
+ *   s4g_get_range   copies the last s4g_range result out (indices [total], sq_dist [total] or NULL); S4G_ERR_STATE when
+ *                   there is none (none after a failed s4g_range).
+ *   _count_dev / _fill_dev: device buffers, enqueued on the context's stream, nothing synchronised.  count writes
+ *   d_offsets [n + 1]; the caller reads d_offsets[n] (= total), allocates, and passes it to fill, which writes the
+ *   sorted lists (d_sq_dist may be NULL).                                                                             */
+int s4g_range(s4g_ctx* ctx, const float* xyz, int n, const float* T_colmajor, float sq_radius, int64_t* offsets,
+              int64_t* total);
+int s4g_get_range(s4g_ctx* ctx, int32_t* indices, float* sq_dist);
+int s4g_range_count_dev(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T_colmajor, float sq_radius,
+                        int64_t* d_offsets);
+int s4g_range_fill_dev(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T_colmajor, float sq_radius,
+                       const int64_t* d_offsets, int64_t total, int32_t* d_indices, float* d_sq_dist);
 /* Verify + the first-maximum rule of TryCongruentSet (algorithms/match4pcsBase.hpp:467-484) in one stream-ordered chain:
  * counts as s4g_verify*, then key = max_k (counts[k] << 32) | (0xFFFFFFFF - index[k])  (index = the candidates' positions
  * in the caller's whole list; NULL = k), then -- when a communicator is attached, s4g_comm_* below -- the maximum over all

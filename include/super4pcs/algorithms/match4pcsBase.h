@@ -71,6 +71,13 @@ class Match4PCSBase {
   /// as delta is; +inf: the nearest point whatever its distance) under the transform that was found (s4g_nearest).
   /// getCorrespondences(nearest, sq_dist, options.delta) equals the two-argument form.
   void getCorrespondences(std::vector<int>* nearest, std::vector<float>* sq_dist, Scalar max_distance) const;
+  /// Every point of getFirstSampled() closer than max_distance (squared in fp32, as delta is; strict: the kd-tree's
+  /// range query) to each point of getSecondSampled() under the transform that was found (s4g_range), in CSR form:
+  /// the list of Q point i is (*indices)[(*offsets)[i] .. (*offsets)[i + 1]), in ascending index, and (*sq_dist) the
+  /// squared distances at the same positions.  Throws std::runtime_error when no registration has run on this object
+  /// or the device call fails (a result the device cannot hold included).
+  void getNeighbors(std::vector<int64_t>* offsets, std::vector<int>* indices, Scalar max_distance,
+                    std::vector<float>* sq_dist = nullptr) const;
 
   /// Approximates the best LCP between P and Q and the rigid motion realising it; on success
   /// Q is replaced by the transformed input.  Returns the LCP in [0,1], or kLargeNumber when Q is

@@ -100,6 +100,8 @@ extern "C" int s4g_create(int device, s4g_ctx** out_ctx) {
   }
   // A/B knob: a fixed number of query patches for Verify instead of the one derived from the L2 size (verify.cu)
   if (const char* e = std::getenv("S4G_VERIFY_PATCHES")) ctx->verify_patches = std::max(0, std::min(kVerifyMaxPatches, std::atoi(e)));
+  // test knob: a smaller window of the per-list sort of s4g_range, so that small results take its multi-chunk path
+  if (const char* e = std::getenv("S4G_RANGE_SORT_WINDOW")) ctx->range_window = std::max(0ll, std::atoll(e));
   {
     // keep freed scratch in the pool instead of returning it to the driver at every synchronisation
     cudaMemPool_t pool = nullptr;
@@ -130,7 +132,8 @@ extern "C" void s4g_destroy(s4g_ctx* ctx) {
                    &ctx->dRms, &ctx->dOk, &ctx->dCandIdx, &ctx->dCounts, &ctx->dResult,
                    &ctx->dMisc, &ctx->bArgs, &ctx->bCounts, &ctx->bPairKeys[0], &ctx->bPairKeys[1], &ctx->bQKeys[0], &ctx->bQKeys[1],
                    &ctx->bQVals[0], &ctx->bQVals[1], &ctx->bQCnt, &ctx->bQuadKeys[0], &ctx->bQuadKeys[1], &ctx->bQuads, &ctx->bMisc,
-                   &ctx->bResults, &ctx->dQpatch, &ctx->dVrec, &ctx->dVsort};
+                   &ctx->bResults, &ctx->dQpatch, &ctx->dVrec, &ctx->dVsort, &ctx->dRangeOff, &ctx->dRangeIdx,
+                   &ctx->dRangeSq};
   for (DevBuf* b : all) free_buf(ctx, *b);
   cudaStreamSynchronize(ctx->stream);
   if (ctx->hPinned) cudaFreeHost(ctx->hPinned);

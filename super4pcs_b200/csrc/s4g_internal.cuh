@@ -199,6 +199,12 @@ struct s4g_ctx {
   DevBuf dQuads;
   long long nQuads = 0;
 
+  // ---- the last s4g_range result (s4g_get_range): offsets [range_n + 1], indices and d^2 [range_total]
+  DevBuf dRangeOff, dRangeIdx, dRangeSq;
+  int range_n = -1;   // -1: none
+  long long range_total = 0;
+  long long range_window = 0;   // largest sort window of s4g_range (S4G_RANGE_SORT_WINDOW when the context was created); 0: none
+
   // ---- several bases per launch chain (s4g_try_bases): shared lists keyed by the base index
   DevBuf bArgs, bCounts, bPairKeys[2], bQKeys[2], bQVals[2], bQCnt, bQuadKeys[2], bQuads, bMisc, bResults;
 

@@ -761,6 +761,130 @@ k_nearest(GridDev g, const float* __restrict__ xyz, int n, const float* __restri
   }
 }
 
+// ---- every P point within a radius, for arbitrary query points (s4g_range): the range query of the reference's kd-tree
+// (KdTree::doQueryDistProcessIndices, kdtree.h:462-514).  One thread per query: y = T x (exact_tq) or x; its list is every
+// original P index j with d^2 < sq_radius (strict: the kd-tree's point test, kdtree.h:485), d^2 computed as in
+// nearest_run_excl.  The lists come out in the order of the search; s4g_range sorts each by j afterwards.
+//
+// Search.  The box descent of k_nearest (NearestQuery, cells_bound, BlockBox) with the fixed bound sq_radius in place of
+// the shrinking best: a box, or a cell row of a block, is dropped when csat says it is empty or when
+// cells_bound(...) >= sq_radius.  The comparison is >=, not the > of k_nearest: cells_bound never exceeds a d^2 the kernel
+// computes (the argument above), so every point of a dropped box or row has d^2 >= sq_radius and is not in the list --
+// a d^2 equal to the radius is excluded here, where k_nearest has to keep it.  Nothing is dropped for any other reason,
+// so the list is exact whatever the order of the descent (children are pushed low half first).  sq_radius <= 0 drops the
+// root (the bound is >= 0); +inf drops nothing that is occupied, and takes every point whose d^2 is finite.
+// Two passes run the identical traversal: kFill = false writes the list's length to offsets[i]; kFill = true writes the
+// list from offsets[i] (their exclusive scan).
+template <bool kFill>
+__global__ void __launch_bounds__(kThreads)
+k_range(GridDev g, const float* __restrict__ xyz, int n, const float* __restrict__ T16, float sq_radius,
+        int64_t* __restrict__ offsets, int32_t* __restrict__ indices, float* __restrict__ sq_dist) {
+  const long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
+  if (i >= n) return;
+  const float4 x = make_float4(__ldg(&xyz[3 * i]), __ldg(&xyz[3 * i + 1]), __ldg(&xyz[3 * i + 2]), 0.f);
+  NearestQuery q;
+  if (T16 != nullptr) {
+    float m[12];
+#pragma unroll
+    for (int e = 0; e < 12; ++e) m[e] = __ldg(&T16[(e & 3) * 4 + (e >> 2)]);
+    exact_tq(m, x, q.tx, q.ty, q.tz);
+  } else {
+    q.tx = x.x;
+    q.ty = x.y;
+    q.tz = x.z;
+  }
+  q.excl = -1;
+  int64_t out = kFill ? offsets[i] : 0;   // fill: the next entry of this list; count: its length so far
+  if (!isnan(q.tx) && !isnan(q.ty) && !isnan(q.tz)) {   // (a NaN coordinate makes every d^2 NaN: the list is empty)
+    const double ih = (double)g.inv_h;
+    q.ux = ((double)q.tx - (double)g.ox) * ih;
+    q.uy = ((double)q.ty - (double)g.oy) * ih;
+    q.uz = ((double)q.tz - (double)g.oz) * ih;
+    q.eps = (double)(max(g.nx, max(g.ny, g.nz)) + 2) * 0x1p-21;
+    q.h2 = 1.0 / (ih * ih);
+    const int cs = g.cshift, mx = g.nx - 1, my = g.ny - 1, mz = g.nz - 1;
+    const BrickShape bs = brick_shape(g);
+    BlockBox stack[kNearestStack];
+    int top = 0;
+    stack[top++] = BlockBox{box_axis(0, g.cnx - 1), box_axis(0, g.cny - 1), box_axis(0, g.cnz - 1)};
+#pragma unroll 1
+    while (top > 0) {
+      const BlockBox b = stack[--top];
+      const int x0 = box_lo(b.x), x1 = box_hi(b.x), y0 = box_lo(b.y), y1 = box_hi(b.y), z0 = box_lo(b.z), z1 = box_hi(b.z);
+      const int cx0 = x0 << cs, cy0 = y0 << cs, cz0 = z0 << cs;
+      const int cx1 = min(((x1 + 1) << cs) - 1, mx), cy1 = min(((y1 + 1) << cs) - 1, my), cz1 = min(((z1 + 1) << cs) - 1, mz);
+      if (cx0 > cx1 || cy0 > cy1 || cz0 > cz1) continue;
+      if (cells_bound(q, cx0, cx1, cy0, cy1, cz0, cz1) >= sq_radius) continue;
+      if (csat_count(g, x0, x1, y0, y1, z0, z1) == 0u) continue;
+      const int ex = x1 - x0, ey = y1 - y0, ez = z1 - z0;
+      if ((ex | ey | ez) != 0) {                       // halve the longest axis
+        BlockBox lo = b, hi = b;
+        if (ex >= ey && ex >= ez) {
+          const int mid = (x0 + x1) >> 1;
+          lo.x = box_axis(x0, mid);
+          hi.x = box_axis(mid + 1, x1);
+        } else if (ey >= ez) {
+          const int mid = (y0 + y1) >> 1;
+          lo.y = box_axis(y0, mid);
+          hi.y = box_axis(mid + 1, y1);
+        } else {
+          const int mid = (z0 + z1) >> 1;
+          lo.z = box_axis(z0, mid);
+          hi.z = box_axis(mid + 1, z1);
+        }
+        stack[top++] = hi;
+        stack[top++] = lo;
+        continue;
+      }
+      // one block: its cell rows within the bound, one contiguous run of sorted points per brick a row crosses
+#pragma unroll 1
+      for (int cz = cz0; cz <= cz1; ++cz)
+#pragma unroll 1
+        for (int cy = cy0; cy <= cy1; ++cy) {
+          if (cells_bound(q, cx0, cx1, cy, cy, cz, cz) >= sq_radius) continue;
+          const int rowb = brick_row(g, bs, cy, cz);
+          const uint32_t rowl = cell_row(bs, cy, cz);
+#pragma unroll 1
+          for (int cx = cx0; cx <= cx1;) {
+            const int xe = min(cx1, cx | bs.m);
+            const int rank = __ldg(&g.top[brick_in_row(bs, rowb, cx)]);
+            if (rank >= 0) {
+              const uint32_t s = __ldg(&g.cellStart[cell_in_row(bs, rank, rowl, cx)]);
+              const uint32_t e = __ldg(&g.cellStart[cell_in_row(bs, rank, rowl, xe) + 1u]);
+#pragma unroll 1
+              for (uint32_t k = s; k < e; ++k) {
+                const float4 p = __ldg(&g.pts[k]);
+                const float dx = __fsub_rn(q.tx, p.x), dy = __fsub_rn(q.ty, p.y), dz = __fsub_rn(q.tz, p.z);
+                const float d2 = __fadd_rn(__fmul_rn(dx, dx), __fadd_rn(__fmul_rn(dy, dy), __fmul_rn(dz, dz)));
+                if (d2 < sq_radius) {
+                  if (kFill) {
+                    indices[out] = __float_as_int(p.w);
+                    if (sq_dist != nullptr) sq_dist[out] = d2;
+                  }
+                  ++out;
+                }
+              }
+            }
+            cx = xe + 1;
+          }
+        }
+    }
+  }
+  if (!kFill) offsets[i] = out;
+}
+
+// the segments of one sort chunk (s4g_range): query i's list is [offsets[i], offsets[i + 1]); the chunk takes the lists
+// that start in [base, base + window), relative to base, and gives every other query an empty segment
+__global__ void k_range_chunk(const int64_t* __restrict__ offsets, int n, int64_t base, int64_t window,
+                              int* __restrict__ begin, int* __restrict__ end) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int64_t b = offsets[i], e = offsets[i + 1];
+  const bool in = b >= base && b < base + window;
+  begin[i] = in ? (int)(b - base) : 0;
+  end[i] = in ? (int)(e - base) : 0;
+}
+
 // column-major 4x4 (16 floats) -> the candidate's record (one thread per candidate)
 __global__ void k_pack_rec(const float* __restrict__ T16, int K, VerifyRecArgs ra, VerifyCand* __restrict__ recs) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1097,4 +1221,174 @@ extern "C" int s4g_nearest_probe_stats(s4g_ctx* ctx, const float* xyz, int n, co
   if (ctx && !out2) { ctx->err = "s4g_nearest_probe_stats: bad arguments"; return S4G_ERR_ARG; }
   if (out2) out2[0] = out2[1] = 0;
   return nearest_host(ctx, "s4g_nearest_probe_stats", xyz, n, T, sq_radius, exclude, index, sq_dist, out2);
+}
+
+static int range_args(s4g_ctx* ctx, const char* who, int n, const void* xyz, float sq_radius, const void* offsets) {
+  if (n < 0 || (n > 0 && (!xyz || !offsets)) || std::isnan(sq_radius)) {
+    ctx->err = std::string(who) + ": bad arguments (n >= 0, xyz and offsets when n > 0, sq_radius not NaN)";
+    return S4G_ERR_ARG;
+  }
+  if (ctx->nP <= 0) {
+    ctx->err = std::string(who) + ": call s4g_set_cloud_p first";
+    return S4G_ERR_STATE;
+  }
+  return S4G_OK;
+}
+
+// enqueue the count pass of k_range and the scan of the lengths: d_offsets [n + 1] = 0, ..., total
+static int range_count(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T, float sq_radius, int64_t* d_offsets) {
+  S4G_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  S4G_CUDA(cudaMemsetAsync(d_offsets + n, 0, sizeof(int64_t), st));
+  k_range<false><<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, 0, st>>>(ctx->grid, d_xyz, n, d_T, sq_radius,
+                                                                                 d_offsets, nullptr, nullptr);
+  ctx->launches++;
+  S4G_CUDA(cudaGetLastError());
+  size_t bytes = 0;
+  S4G_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, bytes, d_offsets, d_offsets, (long long)n + 1, st));
+  S4G_TRY(s4g_reserve(ctx, ctx->dCub, bytes));
+  S4G_CUDA(cub::DeviceScan::ExclusiveSum(ctx->dCub.p, bytes, d_offsets, d_offsets, (long long)n + 1, st));
+  return S4G_OK;
+}
+
+// enqueue the fill pass of k_range into d_indices / d_sq_dist (nullptr: not written) from d_offsets (total = its last
+// entry), then sort every list by index, its d^2 carried along.  CUB's segmented sort addresses the items with int, so the
+// lists are sorted in chunks: chunk c takes the lists that start in the window [c w, (c + 1) w) of the output, and a list
+// that starts there ends before c w + w + |P| <= c w + INT_MAX.  One chunk when total <= INT_MAX.  The sort ping-pongs
+// with a buffer of the chunk's size; when there is more than one chunk, that buffer starts as a copy of the output, so
+// the entries of the neighbouring chunks are copied back unchanged.
+static int range_fill(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T, float sq_radius, const int64_t* d_offsets,
+                      int64_t total, int32_t* d_indices, float* d_sq_dist) {
+  S4G_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  k_range<true><<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, 0, st>>>(
+      ctx->grid, d_xyz, n, d_T, sq_radius, const_cast<int64_t*>(d_offsets), d_indices, d_sq_dist);
+  ctx->launches++;
+  S4G_CUDA(cudaGetLastError());
+  if (total == 0) return S4G_OK;
+  const int64_t kMaxItems = 0x7fffffff;
+  int64_t window = total <= kMaxItems ? total : std::max<int64_t>(1, kMaxItems - ctx->nP);
+  if (ctx->range_window > 0) window = std::min<int64_t>(window, ctx->range_window);
+  const bool chunked = window < total;
+  S4G_TRY(s4g_reserve(ctx, ctx->dScratchD, 2 * (size_t)n * sizeof(int)));
+  int* seg_begin = ctx->dScratchD.as<int>();
+  int* seg_end = seg_begin + n;
+  for (int64_t base = 0; base < total; base += window) {
+    const int len = (int)std::min<int64_t>(total - base, kMaxItems);
+    S4G_TRY(s4g_reserve(ctx, ctx->dScratchB, (size_t)len * sizeof(int32_t)));
+    if (d_sq_dist != nullptr) S4G_TRY(s4g_reserve(ctx, ctx->dScratchC, (size_t)len * sizeof(float)));
+    int32_t* keys = d_indices + base;
+    float* vals = d_sq_dist != nullptr ? d_sq_dist + base : nullptr;
+    if (chunked) {
+      S4G_CUDA(cudaMemcpyAsync(ctx->dScratchB.p, keys, (size_t)len * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+      if (vals != nullptr)
+        S4G_CUDA(cudaMemcpyAsync(ctx->dScratchC.p, vals, (size_t)len * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    }
+    k_range_chunk<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_offsets, n, base, window, seg_begin, seg_end);
+    ctx->launches++;
+    S4G_CUDA(cudaGetLastError());
+    cub::DoubleBuffer<int32_t> dk(keys, ctx->dScratchB.as<int32_t>());
+    cub::DoubleBuffer<float> dv(vals, ctx->dScratchC.as<float>());
+    size_t bytes = 0;
+    if (vals != nullptr) {
+      S4G_CUDA(cub::DeviceSegmentedSort::SortPairs(nullptr, bytes, dk, dv, len, n, seg_begin, seg_end, st));
+      S4G_TRY(s4g_reserve(ctx, ctx->dCub, bytes));
+      S4G_CUDA(cub::DeviceSegmentedSort::SortPairs(ctx->dCub.p, bytes, dk, dv, len, n, seg_begin, seg_end, st));
+    } else {
+      S4G_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, bytes, dk, len, n, seg_begin, seg_end, st));
+      S4G_TRY(s4g_reserve(ctx, ctx->dCub, bytes));
+      S4G_CUDA(cub::DeviceSegmentedSort::SortKeys(ctx->dCub.p, bytes, dk, len, n, seg_begin, seg_end, st));
+    }
+    if (dk.Current() != keys)
+      S4G_CUDA(cudaMemcpyAsync(keys, dk.Current(), (size_t)len * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    if (vals != nullptr && dv.Current() != vals)
+      S4G_CUDA(cudaMemcpyAsync(vals, dv.Current(), (size_t)len * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  }
+  return S4G_OK;
+}
+
+extern "C" int s4g_range_count_dev(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T, float sq_radius,
+                                   int64_t* d_offsets) {
+  if (!ctx) return S4G_ERR_ARG;
+  S4G_TRY(range_args(ctx, "s4g_range_count_dev", n, d_xyz, sq_radius, d_offsets));
+  if (n == 0) {
+    if (d_offsets != nullptr) {
+      S4G_CUDA(cudaSetDevice(ctx->device));
+      S4G_CUDA(cudaMemsetAsync(d_offsets, 0, sizeof(int64_t), ctx->stream));
+    }
+    return S4G_OK;
+  }
+  return range_count(ctx, d_xyz, n, d_T, sq_radius, d_offsets);
+}
+
+extern "C" int s4g_range_fill_dev(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T, float sq_radius,
+                                  const int64_t* d_offsets, int64_t total, int32_t* d_indices, float* d_sq_dist) {
+  if (!ctx) return S4G_ERR_ARG;
+  S4G_TRY(range_args(ctx, "s4g_range_fill_dev", n, d_xyz, sq_radius, d_offsets));
+  if (total < 0 || (n == 0 && total != 0) || (total > 0 && !d_indices)) {
+    ctx->err = "s4g_range_fill_dev: bad arguments (total = d_offsets[n] >= 0, indices when total > 0)";
+    return S4G_ERR_ARG;
+  }
+  if (n == 0) return S4G_OK;
+  return range_fill(ctx, d_xyz, n, d_T, sq_radius, d_offsets, total, d_indices, d_sq_dist);
+}
+
+extern "C" int s4g_range(s4g_ctx* ctx, const float* xyz, int n, const float* T, float sq_radius, int64_t* offsets,
+                         int64_t* total) {
+  if (!ctx) return S4G_ERR_ARG;
+  ctx->range_n = -1;   // a failed call leaves no result
+  ctx->range_total = 0;
+  S4G_TRY(range_args(ctx, "s4g_range", n, xyz, sq_radius, offsets));
+  if (!offsets || !total) {
+    ctx->err = "s4g_range: bad arguments (offsets and total)";
+    return S4G_ERR_ARG;
+  }
+  if (n == 0) {
+    offsets[0] = 0;
+    *total = 0;
+    ctx->range_n = 0;
+    return S4G_OK;
+  }
+  S4G_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  const size_t nn = (size_t)n;
+  S4G_TRY(s4g_reserve(ctx, ctx->dScratchA, nn * 3 * sizeof(float) + 16 * sizeof(float)));
+  S4G_TRY(s4g_reserve(ctx, ctx->dRangeOff, (nn + 1) * sizeof(int64_t)));
+  float* d_xyz = ctx->dScratchA.as<float>();
+  float* d_T = T != nullptr ? d_xyz + nn * 3 : nullptr;
+  S4G_CUDA(cudaMemcpyAsync(d_xyz, xyz, nn * 3 * sizeof(float), cudaMemcpyHostToDevice, st));
+  if (T != nullptr) S4G_CUDA(cudaMemcpyAsync(d_T, T, 16 * sizeof(float), cudaMemcpyHostToDevice, st));
+  int64_t* d_off = ctx->dRangeOff.as<int64_t>();
+  S4G_TRY(range_count(ctx, d_xyz, n, d_T, sq_radius, d_off));
+  S4G_CUDA(cudaMemcpyAsync(offsets, d_off, (nn + 1) * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  S4G_CUDA(cudaStreamSynchronize(st));
+  const int64_t tot = offsets[n];
+  S4G_TRY(s4g_reserve(ctx, ctx->dRangeIdx, (size_t)std::max<int64_t>(tot, 1) * sizeof(int32_t)));
+  S4G_TRY(s4g_reserve(ctx, ctx->dRangeSq, (size_t)std::max<int64_t>(tot, 1) * sizeof(float)));
+  S4G_TRY(range_fill(ctx, d_xyz, n, d_T, sq_radius, d_off, tot, ctx->dRangeIdx.as<int32_t>(), ctx->dRangeSq.as<float>()));
+  S4G_CUDA(cudaStreamSynchronize(st));
+  ctx->range_n = n;
+  ctx->range_total = tot;
+  *total = tot;
+  return S4G_OK;
+}
+
+extern "C" int s4g_get_range(s4g_ctx* ctx, int32_t* indices, float* sq_dist) {
+  if (!ctx) return S4G_ERR_ARG;
+  if (ctx->range_n < 0) {
+    ctx->err = "s4g_get_range: no s4g_range result";
+    return S4G_ERR_STATE;
+  }
+  const size_t tot = (size_t)ctx->range_total;
+  if (tot == 0) return S4G_OK;
+  if (!indices) {
+    ctx->err = "s4g_get_range: null indices";
+    return S4G_ERR_ARG;
+  }
+  S4G_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = ctx->stream;
+  S4G_CUDA(cudaMemcpyAsync(indices, ctx->dRangeIdx.p, tot * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  if (sq_dist != nullptr) S4G_CUDA(cudaMemcpyAsync(sq_dist, ctx->dRangeSq.p, tot * sizeof(float), cudaMemcpyDeviceToHost, st));
+  S4G_CUDA(cudaStreamSynchronize(st));
+  return S4G_OK;
 }

@@ -96,6 +96,10 @@ def load_library():
         "s4g_nearest": ([vp, vp, i32, vp, f32, vp, vp, vp], i32),
         "s4g_nearest_dev": ([vp, vp, i32, vp, f32, vp, vp, vp], i32),
         "s4g_nearest_probe_stats": ([vp, vp, i32, vp, f32, vp, vp, vp, vp], i32),
+        "s4g_range": ([vp, vp, i32, vp, f32, vp, vp], i32),
+        "s4g_get_range": ([vp, vp, vp], i32),
+        "s4g_range_count_dev": ([vp, vp, i32, vp, f32, vp], i32),
+        "s4g_range_fill_dev": ([vp, vp, i32, vp, f32, vp, i64, vp, vp], i32),
         "s4g_verify_best_dev": ([vp, vp, i32, vp, vp, vp], i32),
         "s4g_verify_best": ([vp, vp, i32, vp, vp, vp], i32),
         "s4g_comm_unique_id": ([vp], i32),
@@ -287,6 +291,34 @@ class Context:
         v = lambda p: C.c_void_p(p) if p else None  # noqa: E731
         self._chk(self._L.s4g_nearest_dev(self.h, v(d_xyz_ptr), int(n), v(d_T_ptr), float(sq_radius), v(d_exclude_ptr),
                                           v(d_index_ptr), v(d_sq_dist_ptr)))
+
+    def range_query(self, xyz, sq_radius, T=None):
+        """-> (offsets [n + 1] int64, indices [total] int32, sq_dist [total] float32): for every query point x, every
+        resident P point j with d^2 = |T x - p_j|^2 < sq_radius (x when T is None), in ascending j; list i is
+        indices[offsets[i]:offsets[i + 1]].  See s4g.h (s4g_range)."""
+        xyz = _c(xyz).reshape(-1, 3)
+        n = len(xyz)
+        T = None if T is None else _c(T).reshape(16)
+        offsets = np.zeros(n + 1, np.int64)
+        total = C.c_int64(0)
+        self._chk(self._L.s4g_range(self.h, _p(xyz), n, _p(T), float(sq_radius), _p(offsets), C.byref(total)))
+        indices, sq = np.empty(total.value, np.int32), np.empty(total.value, _f)
+        self._chk(self._L.s4g_get_range(self.h, _p(indices), _p(sq)))
+        return offsets, indices, sq
+
+    def range_count_dev(self, d_xyz_ptr, n, d_offsets_ptr, sq_radius, d_T_ptr=None):
+        """device pointers (n x 3 float32 queries, n + 1 int64 offsets, 16 float32 T or None): the CSR offsets of the
+        range query, stream-ordered, nothing synchronised; the total is d_offsets[n]"""
+        v = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        self._chk(self._L.s4g_range_count_dev(self.h, v(d_xyz_ptr), int(n), v(d_T_ptr), float(sq_radius),
+                                              v(d_offsets_ptr)))
+
+    def range_fill_dev(self, d_xyz_ptr, n, d_offsets_ptr, total, d_indices_ptr, d_sq_dist_ptr, sq_radius, d_T_ptr=None):
+        """device pointers (the queries and offsets given to range_count_dev, total = d_offsets[n]; total int32 indices,
+        total float32 d^2 or None): the sorted lists, stream-ordered, nothing synchronised"""
+        v = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        self._chk(self._L.s4g_range_fill_dev(self.h, v(d_xyz_ptr), int(n), v(d_T_ptr), float(sq_radius), v(d_offsets_ptr),
+                                             int(total), v(d_indices_ptr), v(d_sq_dist_ptr)))
 
     def verify_best_dev(self, d_T_ptr, K, d_index_ptr, d_counts_ptr, d_key_ptr):
         """Verify + first-maximum key (+ the maximum over the communicator's ranks), stream-ordered, nothing synchronised"""
