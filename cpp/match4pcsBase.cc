@@ -458,6 +458,25 @@ void Match4PCSBase::getNeighbors(std::vector<int64_t>* offsets, std::vector<int>
     ThrowLaneError(gpu_, "s4g_get_range");
 }
 
+void Match4PCSBase::getKNearest(std::vector<int>* indices, std::vector<float>* sq_dist, int k, Scalar max_distance) const {
+  if (gpu_ == nullptr || sampled_P_3D_.empty() || sampled_Q_3D_.empty())
+    throw std::runtime_error("super4pcs-b200: getKNearest: no registration has run on this matcher");
+  if (indices == nullptr) throw std::invalid_argument("super4pcs-b200: getKNearest: null output");
+  if (std::isnan(max_distance)) throw std::invalid_argument("super4pcs-b200: getKNearest: max_distance is NaN");
+  const MatrixType T = transform_;
+  const int n = int(sampled_Q_3D_.size());
+  std::vector<float> xyz(3 * size_t(n));
+  for (int i = 0; i < n; ++i)
+    for (int c = 0; c < 3; ++c) xyz[3 * size_t(i) + c] = sampled_Q_3D_[i].pos()[c];
+  const size_t entries = k > 0 ? size_t(n) * size_t(k) : 0;
+  indices->resize(entries);
+  if (sq_dist) sq_dist->resize(entries);
+  const float sq_radius = max_distance * max_distance;   // as getCorrespondences squares it
+  if (s4g_knn(gpu_, xyz.data(), n, T.data(), k, sq_radius, nullptr, reinterpret_cast<int32_t*>(indices->data()),
+              sq_dist ? sq_dist->data() : nullptr) != S4G_OK)
+    ThrowLaneError(gpu_, "s4g_knn");
+}
+
 bool Match4PCSBase::TryBaseOnLane(s4g_ctx*, const SelectedBase&, DeviceBest*) const { return false; }
 
 bool Match4PCSBase::TryBasesOnLane(s4g_ctx*, const std::vector<SelectedBase*>&) const { return false; }

@@ -128,6 +128,23 @@ int s4g_nearest_dev(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T_co
                     const int32_t* d_exclude, int32_t* d_index, float* d_sq_dist);
 int s4g_nearest_probe_stats(s4g_ctx* ctx, const float* xyz, int n, const float* T_colmajor, float sq_radius,
                             const int32_t* exclude, int32_t* index, float* sq_dist, uint64_t* out2);
+/* The k nearest neighbours on the resident sampled P, for n arbitrary query points xyz (n x 3).  Row i is
+ * index[i*k .. i*k+k) / sq_dist[i*k .. i*k+k) (64-bit offsets: n*k may exceed 2^31): the k lexicographically smallest
+ * (d^2, j) over the P points with d^2 = |y_i - p_j|^2 <= sq_radius and j != exclude[i], in ascending (d^2, j); y_i, d^2
+ * and j as in s4g_nearest (sq_dist bit for bit what it computes).  A row with fewer such points is padded at its end with
+ * index -1 and sq_dist +inf; a query with a NaN coordinate gets a row of padding.  k = 1 is s4g_nearest bit for bit.  For
+ * a finite radius, row i is the first k entries of the s4g_range list at nextafterf(sq_radius, +inf) with j = exclude[i]
+ * removed, ordered by (d^2, j).  1 <= k <= 64, sq_radius any value but NaN (+inf = unbounded), exclude NULL or n entries
+ * (-1 = none); otherwise S4G_ERR_ARG.  Needs s4g_set_cloud_p only (S4G_ERR_STATE before it); n == 0 is a no-op; an
+ * output the device cannot stage -> S4G_ERR_NOMEM.  sq_dist may be NULL.
+ * _dev: device buffers, enqueued on the context's stream, nothing synchronised.
+ * _probe_stats: as s4g_knn, and out2 = {P points tested, coarse blocks scanned} summed over the queries.              */
+int s4g_knn(s4g_ctx* ctx, const float* xyz, int n, const float* T_colmajor, int k, float sq_radius,
+            const int32_t* exclude, int32_t* index, float* sq_dist);
+int s4g_knn_dev(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T_colmajor, int k, float sq_radius,
+                const int32_t* d_exclude, int32_t* d_index, float* d_sq_dist);
+int s4g_knn_probe_stats(s4g_ctx* ctx, const float* xyz, int n, const float* T_colmajor, int k, float sq_radius,
+                        const int32_t* exclude, int32_t* index, float* sq_dist, uint64_t* out2);
 /* The range query of the reference's kd-tree (KdTree::doQueryDist / doQueryDistIndices / doQueryDistProcessIndices,
  * accelerators/kdtree.h:231-262, body :462-514) on the resident sampled P, for n arbitrary query points xyz (n x 3):
  * the list of query i is every j with d^2 = |y_i - p_j|^2 < sq_radius (strict, the kd-tree's point test kdtree.h:485),

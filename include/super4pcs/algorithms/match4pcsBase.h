@@ -17,6 +17,7 @@
 #include <cstdint>
 #include <deque>
 #include <exception>
+#include <limits>
 #include <map>
 #include <random>
 #include <utility>
@@ -78,6 +79,13 @@ class Match4PCSBase {
   /// or the device call fails (a result the device cannot hold included).
   void getNeighbors(std::vector<int64_t>* offsets, std::vector<int>* indices, Scalar max_distance,
                     std::vector<float>* sq_dist = nullptr) const;
+  /// The k nearest points of getFirstSampled() with distance <= max_distance (squared in fp32, as delta is; +inf:
+  /// unbounded) to each point of getSecondSampled() under the transform that was found (s4g_knn): row i is
+  /// (*indices)[i * k .. i * k + k), in ascending (squared distance, index), padded at its end with -1 (and +inf in
+  /// *sq_dist, which may be null) when fewer points lie within max_distance.  1 <= k <= 64.  Throws std::runtime_error
+  /// when no registration has run on this object or the device call fails (a bad k included).
+  void getKNearest(std::vector<int>* indices, std::vector<float>* sq_dist, int k,
+                   Scalar max_distance = std::numeric_limits<Scalar>::infinity()) const;
 
   /// Approximates the best LCP between P and Q and the rigid motion realising it; on success
   /// Q is replaced by the transformed input.  Returns the LCP in [0,1], or kLargeNumber when Q is

@@ -885,6 +885,160 @@ __global__ void k_range_chunk(const int64_t* __restrict__ offsets, int n, int64_
   end[i] = in ? (int)(e - base) : 0;
 }
 
+// ---- the k nearest P points within a radius, for arbitrary query points (s4g_knn).  One thread per query: y = T x
+// (exact_tq) or x; its row is the k lexicographically smallest (d^2, original P index j) over the P points with
+// d^2 <= sq_radius and j != exclude, ascending, d^2 computed as in nearest_run_excl; a row with fewer such points is
+// padded with (-1, +inf).  k = 1 is k_nearest's answer.
+//
+// Search.  The box descent of k_nearest (NearestQuery, cells_bound, BlockBox, csat) with one change: the bound is
+// sq_radius while fewer than k points are held, and the d^2 of the k-th held entry once k are.  A box or cell row is
+// dropped when its cells_bound is strictly above the bound, as in k_nearest.  A point is inserted when d^2 <= sq_radius,
+// j != exclude and (d^2, j) is below the k-th held entry (a NaN d^2 fails the first test and is never taken).
+// Determinism.  cells_bound never exceeds a d^2 the kernel computes (the argument above k_nearest), so every point of a
+// dropped box or row has d^2 > bound: beyond the radius while the row is not full, and after that above the k-th held
+// d^2, which only decreases -- such a point is above the final k-th entry too, so it could be neither in the row nor tie
+// with its last entry.  A point at exactly the k-th distance with a smaller j is never dropped (the test is strict) and
+// displaces the entry with the larger j.  Every other point is compared with the held list, and every P point is binned
+// in one cell, so it is seen once: the row is the lexicographic k-minimum whatever the order of the search.
+// Storage.  The held entries are 64-bit keys (d^2 bits << 32 | j), which order as (d^2, j) because d^2 is never negative
+// nor NaN; kEmpty, above every key, marks a free slot.  They sit in a per-thread array of kCap slots, sorted ascending
+// (local memory: it is indexed by the run-time k), and an insertion shifts the larger keys up by one.  kCap is k rounded
+// up to 8, 16, 32 or 64, so that a small k does not carry the stack frame of the largest.  The descent loop and the row
+// walk are written out here as in k_range: folding k_nearest's into a shared template moves one instruction of its SASS.
+constexpr unsigned long long kEmpty = ~0ull;
+
+template <int kCap, bool kStats>
+__global__ void __launch_bounds__(kThreads)
+k_knn(GridDev g, const float* __restrict__ xyz, int n, const float* __restrict__ T16, int k, float sq_radius,
+      const int32_t* __restrict__ exclude, int32_t* __restrict__ index, float* __restrict__ sq_dist,
+      unsigned long long* __restrict__ stats) {
+  const long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
+  NearestStats st;
+  if (i < n) {
+    const float4 x = make_float4(__ldg(&xyz[3 * i]), __ldg(&xyz[3 * i + 1]), __ldg(&xyz[3 * i + 2]), 0.f);
+    NearestQuery q;
+    if (T16 != nullptr) {
+      float m[12];
+#pragma unroll
+      for (int e = 0; e < 12; ++e) m[e] = __ldg(&T16[(e & 3) * 4 + (e >> 2)]);
+      exact_tq(m, x, q.tx, q.ty, q.tz);
+    } else {
+      q.tx = x.x;
+      q.ty = x.y;
+      q.tz = x.z;
+    }
+    q.excl = exclude != nullptr ? __ldg(&exclude[i]) : -1;
+    unsigned long long held[kCap];
+#pragma unroll 1
+    for (int e = 0; e < k; ++e) held[e] = kEmpty;
+    unsigned long long kth = kEmpty;   // held[k - 1]
+    float bound = sq_radius;
+    if (!isnan(q.tx) && !isnan(q.ty) && !isnan(q.tz)) {   // (a NaN coordinate makes every d^2 NaN: nothing is taken)
+      const double ih = (double)g.inv_h;
+      q.ux = ((double)q.tx - (double)g.ox) * ih;
+      q.uy = ((double)q.ty - (double)g.oy) * ih;
+      q.uz = ((double)q.tz - (double)g.oz) * ih;
+      q.eps = (double)(max(g.nx, max(g.ny, g.nz)) + 2) * 0x1p-21;
+      q.h2 = 1.0 / (ih * ih);
+      const int cs = g.cshift, mx = g.nx - 1, my = g.ny - 1, mz = g.nz - 1;
+      const BrickShape bs = brick_shape(g);
+      BlockBox stack[kNearestStack];
+      int top = 0;
+      stack[top++] = BlockBox{box_axis(0, g.cnx - 1), box_axis(0, g.cny - 1), box_axis(0, g.cnz - 1)};
+#pragma unroll 1
+      while (top > 0) {
+        const BlockBox b = stack[--top];
+        const int x0 = box_lo(b.x), x1 = box_hi(b.x), y0 = box_lo(b.y), y1 = box_hi(b.y), z0 = box_lo(b.z), z1 = box_hi(b.z);
+        const int cx0 = x0 << cs, cy0 = y0 << cs, cz0 = z0 << cs;
+        const int cx1 = min(((x1 + 1) << cs) - 1, mx), cy1 = min(((y1 + 1) << cs) - 1, my), cz1 = min(((z1 + 1) << cs) - 1, mz);
+        if (cx0 > cx1 || cy0 > cy1 || cz0 > cz1) continue;
+        if (cells_bound(q, cx0, cx1, cy0, cy1, cz0, cz1) > bound) continue;
+        if (csat_count(g, x0, x1, y0, y1, z0, z1) == 0u) continue;
+        const int ex = x1 - x0, ey = y1 - y0, ez = z1 - z0;
+        if ((ex | ey | ez) != 0) {                       // halve the longest axis, the nearer half searched first
+          BlockBox lo = b, hi = b;
+          bool lo_near;
+          if (ex >= ey && ex >= ez) {
+            const int mid = (x0 + x1) >> 1;
+            lo.x = box_axis(x0, mid);
+            hi.x = box_axis(mid + 1, x1);
+            lo_near = q.ux < (double)((mid + 1) << cs);
+          } else if (ey >= ez) {
+            const int mid = (y0 + y1) >> 1;
+            lo.y = box_axis(y0, mid);
+            hi.y = box_axis(mid + 1, y1);
+            lo_near = q.uy < (double)((mid + 1) << cs);
+          } else {
+            const int mid = (z0 + z1) >> 1;
+            lo.z = box_axis(z0, mid);
+            hi.z = box_axis(mid + 1, z1);
+            lo_near = q.uz < (double)((mid + 1) << cs);
+          }
+          stack[top++] = lo_near ? hi : lo;
+          stack[top++] = lo_near ? lo : hi;
+          continue;
+        }
+        // one block: its cell rows within the bound, one contiguous run of sorted points per brick a row crosses
+        if (kStats) st.blocks++;
+#pragma unroll 1
+        for (int cz = cz0; cz <= cz1; ++cz)
+#pragma unroll 1
+          for (int cy = cy0; cy <= cy1; ++cy) {
+            if (cells_bound(q, cx0, cx1, cy, cy, cz, cz) > bound) continue;
+            const int rowb = brick_row(g, bs, cy, cz);
+            const uint32_t rowl = cell_row(bs, cy, cz);
+#pragma unroll 1
+            for (int cx = cx0; cx <= cx1;) {
+              const int xe = min(cx1, cx | bs.m);
+              const int rank = __ldg(&g.top[brick_in_row(bs, rowb, cx)]);
+              if (rank >= 0) {
+                const uint32_t s = __ldg(&g.cellStart[cell_in_row(bs, rank, rowl, cx)]);
+                const uint32_t e = __ldg(&g.cellStart[cell_in_row(bs, rank, rowl, xe) + 1u]);
+                if (kStats) st.tested += e - s;
+#pragma unroll 1
+                for (uint32_t t = s; t < e; ++t) {
+                  const float4 p = __ldg(&g.pts[t]);
+                  const float dx = __fsub_rn(q.tx, p.x), dy = __fsub_rn(q.ty, p.y), dz = __fsub_rn(q.tz, p.z);
+                  const float d2 = __fadd_rn(__fmul_rn(dx, dx), __fadd_rn(__fmul_rn(dy, dy), __fmul_rn(dz, dz)));
+                  const int j = __float_as_int(p.w);
+                  if (!(d2 <= sq_radius) || j == q.excl) continue;
+                  const unsigned long long key = ((unsigned long long)__float_as_uint(d2) << 32) | (uint32_t)j;
+                  if (key >= kth) continue;
+                  int at = k - 1;
+#pragma unroll 1
+                  for (; at > 0 && held[at - 1] > key; --at) held[at] = held[at - 1];
+                  held[at] = key;
+                  kth = held[k - 1];
+                  if (kth != kEmpty) bound = __uint_as_float((uint32_t)(kth >> 32));
+                }
+              }
+              cx = xe + 1;
+            }
+          }
+      }
+    }
+    const long long row = i * (long long)k;
+#pragma unroll 1
+    for (int e = 0; e < k; ++e) {
+      const unsigned long long key = held[e];
+      index[row + e] = key != kEmpty ? (int32_t)(uint32_t)key : -1;
+      if (sq_dist != nullptr)
+        sq_dist[row + e] = key != kEmpty ? __uint_as_float((uint32_t)(key >> 32)) : __int_as_float(0x7f800000);
+    }
+  }
+  if (kStats) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      st.tested += __shfl_down_sync(0xffffffffu, st.tested, o);
+      st.blocks += __shfl_down_sync(0xffffffffu, st.blocks, o);
+    }
+    if ((threadIdx.x & 31) == 0) {
+      atomicAdd(&stats[0], st.tested);
+      atomicAdd(&stats[1], st.blocks);
+    }
+  }
+}
+
 // column-major 4x4 (16 floats) -> the candidate's record (one thread per candidate)
 __global__ void k_pack_rec(const float* __restrict__ T16, int K, VerifyRecArgs ra, VerifyCand* __restrict__ recs) {
   const int k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1175,18 +1329,18 @@ extern "C" int s4g_nearest_dev(s4g_ctx* ctx, const float* d_xyz, int n, const fl
   return launch_nearest(ctx, d_xyz, n, d_T, sq_radius, d_exclude, d_index, d_sq_dist, nullptr);
 }
 
-// host buffers -> the context's scratch, k_nearest, back; stats: nullptr or the two counters of the statistics variant
-static int nearest_host(s4g_ctx* ctx, const char* who, const float* xyz, int n, const float* T, float sq_radius,
-                        const int32_t* exclude, int32_t* index, float* sq_dist, uint64_t* stats) {
-  if (!ctx) return S4G_ERR_ARG;
-  S4G_TRY(nearest_args(ctx, who, n, xyz, sq_radius, index));
-  if (n == 0) return S4G_OK;
+// host buffers -> the context's scratch, launch(d_xyz, d_T, d_exclude, d_index, d_sq_dist, d_stats), back: the staging of
+// s4g_nearest and s4g_knn, whose outputs have `width` entries per query.  stats: nullptr or the two counters of the
+// statistics variant.  The arguments are checked by the caller, and n > 0.
+template <class Launch>
+static int query_host(s4g_ctx* ctx, const float* xyz, int n, const float* T, int width, const int32_t* exclude,
+                      int32_t* index, float* sq_dist, uint64_t* stats, Launch launch) {
   S4G_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = ctx->stream;
-  const size_t nn = (size_t)n;
+  const size_t nn = (size_t)n, nw = nn * (size_t)width;
   S4G_TRY(s4g_reserve(ctx, ctx->dScratchA, nn * 3 * sizeof(float) + 16 * sizeof(float)));
-  S4G_TRY(s4g_reserve(ctx, ctx->dScratchB, nn * sizeof(int32_t)));
-  if (sq_dist != nullptr) S4G_TRY(s4g_reserve(ctx, ctx->dScratchC, nn * sizeof(float)));
+  S4G_TRY(s4g_reserve(ctx, ctx->dScratchB, nw * sizeof(int32_t)));
+  if (sq_dist != nullptr) S4G_TRY(s4g_reserve(ctx, ctx->dScratchC, nw * sizeof(float)));
   if (exclude != nullptr) S4G_TRY(s4g_reserve(ctx, ctx->dScratchD, nn * sizeof(int32_t)));
   if (stats != nullptr) S4G_TRY(s4g_reserve(ctx, ctx->dMisc, 256));
   float* d_xyz = ctx->dScratchA.as<float>();
@@ -1196,11 +1350,11 @@ static int nearest_host(s4g_ctx* ctx, const char* who, const float* xyz, int n, 
   if (exclude != nullptr)
     S4G_CUDA(cudaMemcpyAsync(ctx->dScratchD.p, exclude, nn * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   if (stats != nullptr) S4G_CUDA(cudaMemsetAsync(ctx->dMisc.p, 0, 2 * sizeof(unsigned long long), st));
-  S4G_TRY(launch_nearest(ctx, d_xyz, n, d_T, sq_radius, exclude != nullptr ? ctx->dScratchD.as<int32_t>() : nullptr,
-                         ctx->dScratchB.as<int32_t>(), sq_dist != nullptr ? ctx->dScratchC.as<float>() : nullptr,
-                         stats != nullptr ? ctx->dMisc.as<unsigned long long>() : nullptr));
-  S4G_CUDA(cudaMemcpyAsync(index, ctx->dScratchB.p, nn * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  if (sq_dist != nullptr) S4G_CUDA(cudaMemcpyAsync(sq_dist, ctx->dScratchC.p, nn * sizeof(float), cudaMemcpyDeviceToHost, st));
+  S4G_TRY(launch(d_xyz, d_T, exclude != nullptr ? ctx->dScratchD.as<int32_t>() : nullptr, ctx->dScratchB.as<int32_t>(),
+                 sq_dist != nullptr ? ctx->dScratchC.as<float>() : nullptr,
+                 stats != nullptr ? ctx->dMisc.as<unsigned long long>() : nullptr));
+  S4G_CUDA(cudaMemcpyAsync(index, ctx->dScratchB.p, nw * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  if (sq_dist != nullptr) S4G_CUDA(cudaMemcpyAsync(sq_dist, ctx->dScratchC.p, nw * sizeof(float), cudaMemcpyDeviceToHost, st));
   unsigned long long h[2] = {0, 0};
   if (stats != nullptr) S4G_CUDA(cudaMemcpyAsync(h, ctx->dMisc.p, sizeof h, cudaMemcpyDeviceToHost, st));
   S4G_CUDA(cudaStreamSynchronize(st));
@@ -1209,6 +1363,19 @@ static int nearest_host(s4g_ctx* ctx, const char* who, const float* xyz, int n, 
     stats[1] = h[1];
   }
   return S4G_OK;
+}
+
+// host buffers -> the context's scratch, k_nearest, back; stats: nullptr or the two counters of the statistics variant
+static int nearest_host(s4g_ctx* ctx, const char* who, const float* xyz, int n, const float* T, float sq_radius,
+                        const int32_t* exclude, int32_t* index, float* sq_dist, uint64_t* stats) {
+  if (!ctx) return S4G_ERR_ARG;
+  S4G_TRY(nearest_args(ctx, who, n, xyz, sq_radius, index));
+  if (n == 0) return S4G_OK;
+  return query_host(ctx, xyz, n, T, 1, exclude, index, sq_dist, stats,
+                    [&](const float* d_xyz, const float* d_T, const int32_t* d_excl, int32_t* d_index, float* d_sq,
+                        unsigned long long* d_stats) {
+                      return launch_nearest(ctx, d_xyz, n, d_T, sq_radius, d_excl, d_index, d_sq, d_stats);
+                    });
 }
 
 extern "C" int s4g_nearest(s4g_ctx* ctx, const float* xyz, int n, const float* T, float sq_radius, const int32_t* exclude,
@@ -1221,6 +1388,78 @@ extern "C" int s4g_nearest_probe_stats(s4g_ctx* ctx, const float* xyz, int n, co
   if (ctx && !out2) { ctx->err = "s4g_nearest_probe_stats: bad arguments"; return S4G_ERR_ARG; }
   if (out2) out2[0] = out2[1] = 0;
   return nearest_host(ctx, "s4g_nearest_probe_stats", xyz, n, T, sq_radius, exclude, index, sq_dist, out2);
+}
+
+constexpr int kKnnMax = 64;   // the largest k of s4g_knn (the slots of k_knn's widest instance)
+
+static int knn_args(s4g_ctx* ctx, const char* who, int n, const void* xyz, int k, float sq_radius, const void* index) {
+  if (k < 1 || k > kKnnMax) {
+    ctx->err = std::string(who) + ": bad arguments (1 <= k <= 64)";
+    return S4G_ERR_ARG;
+  }
+  return nearest_args(ctx, who, n, xyz, sq_radius, index);
+}
+
+// enqueue k_knn on the context's stream: the instance whose slots are k rounded up to 8, 16, 32 or 64 (stats != nullptr:
+// the statistics variant)
+template <int kCap>
+static void launch_knn_cap(s4g_ctx* ctx, unsigned nblk, const float* d_xyz, int n, const float* d_T, int k, float sq_radius,
+                           const int32_t* d_exclude, int32_t* d_index, float* d_sq_dist, unsigned long long* stats) {
+  if (stats != nullptr)
+    k_knn<kCap, true><<<nblk, kThreads, 0, ctx->stream>>>(ctx->grid, d_xyz, n, d_T, k, sq_radius, d_exclude, d_index,
+                                                          d_sq_dist, stats);
+  else
+    k_knn<kCap, false><<<nblk, kThreads, 0, ctx->stream>>>(ctx->grid, d_xyz, n, d_T, k, sq_radius, d_exclude, d_index,
+                                                           d_sq_dist, nullptr);
+}
+
+static int launch_knn(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T, int k, float sq_radius,
+                      const int32_t* d_exclude, int32_t* d_index, float* d_sq_dist, unsigned long long* stats) {
+  S4G_CUDA(cudaSetDevice(ctx->device));
+  const unsigned nblk = (unsigned)((n + kThreads - 1) / kThreads);
+  if (k <= 8)
+    launch_knn_cap<8>(ctx, nblk, d_xyz, n, d_T, k, sq_radius, d_exclude, d_index, d_sq_dist, stats);
+  else if (k <= 16)
+    launch_knn_cap<16>(ctx, nblk, d_xyz, n, d_T, k, sq_radius, d_exclude, d_index, d_sq_dist, stats);
+  else if (k <= 32)
+    launch_knn_cap<32>(ctx, nblk, d_xyz, n, d_T, k, sq_radius, d_exclude, d_index, d_sq_dist, stats);
+  else
+    launch_knn_cap<kKnnMax>(ctx, nblk, d_xyz, n, d_T, k, sq_radius, d_exclude, d_index, d_sq_dist, stats);
+  ctx->launches++;
+  S4G_CUDA(cudaGetLastError());
+  return S4G_OK;
+}
+
+extern "C" int s4g_knn_dev(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T, int k, float sq_radius,
+                           const int32_t* d_exclude, int32_t* d_index, float* d_sq_dist) {
+  if (!ctx) return S4G_ERR_ARG;
+  S4G_TRY(knn_args(ctx, "s4g_knn_dev", n, d_xyz, k, sq_radius, d_index));
+  if (n == 0) return S4G_OK;
+  return launch_knn(ctx, d_xyz, n, d_T, k, sq_radius, d_exclude, d_index, d_sq_dist, nullptr);
+}
+
+static int knn_host(s4g_ctx* ctx, const char* who, const float* xyz, int n, const float* T, int k, float sq_radius,
+                    const int32_t* exclude, int32_t* index, float* sq_dist, uint64_t* stats) {
+  if (!ctx) return S4G_ERR_ARG;
+  S4G_TRY(knn_args(ctx, who, n, xyz, k, sq_radius, index));
+  if (n == 0) return S4G_OK;
+  return query_host(ctx, xyz, n, T, k, exclude, index, sq_dist, stats,
+                    [&](const float* d_xyz, const float* d_T, const int32_t* d_excl, int32_t* d_index, float* d_sq,
+                        unsigned long long* d_stats) {
+                      return launch_knn(ctx, d_xyz, n, d_T, k, sq_radius, d_excl, d_index, d_sq, d_stats);
+                    });
+}
+
+extern "C" int s4g_knn(s4g_ctx* ctx, const float* xyz, int n, const float* T, int k, float sq_radius,
+                       const int32_t* exclude, int32_t* index, float* sq_dist) {
+  return knn_host(ctx, "s4g_knn", xyz, n, T, k, sq_radius, exclude, index, sq_dist, nullptr);
+}
+
+extern "C" int s4g_knn_probe_stats(s4g_ctx* ctx, const float* xyz, int n, const float* T, int k, float sq_radius,
+                                   const int32_t* exclude, int32_t* index, float* sq_dist, uint64_t* out2) {
+  if (ctx && !out2) { ctx->err = "s4g_knn_probe_stats: bad arguments"; return S4G_ERR_ARG; }
+  if (out2) out2[0] = out2[1] = 0;
+  return knn_host(ctx, "s4g_knn_probe_stats", xyz, n, T, k, sq_radius, exclude, index, sq_dist, out2);
 }
 
 static int range_args(s4g_ctx* ctx, const char* who, int n, const void* xyz, float sq_radius, const void* offsets) {

@@ -96,6 +96,9 @@ def load_library():
         "s4g_nearest": ([vp, vp, i32, vp, f32, vp, vp, vp], i32),
         "s4g_nearest_dev": ([vp, vp, i32, vp, f32, vp, vp, vp], i32),
         "s4g_nearest_probe_stats": ([vp, vp, i32, vp, f32, vp, vp, vp, vp], i32),
+        "s4g_knn": ([vp, vp, i32, vp, i32, f32, vp, vp, vp], i32),
+        "s4g_knn_dev": ([vp, vp, i32, vp, i32, f32, vp, vp, vp], i32),
+        "s4g_knn_probe_stats": ([vp, vp, i32, vp, i32, f32, vp, vp, vp, vp], i32),
         "s4g_range": ([vp, vp, i32, vp, f32, vp, vp], i32),
         "s4g_get_range": ([vp, vp, vp], i32),
         "s4g_range_count_dev": ([vp, vp, i32, vp, f32, vp], i32),
@@ -291,6 +294,31 @@ class Context:
         v = lambda p: C.c_void_p(p) if p else None  # noqa: E731
         self._chk(self._L.s4g_nearest_dev(self.h, v(d_xyz_ptr), int(n), v(d_T_ptr), float(sq_radius), v(d_exclude_ptr),
                                           v(d_index_ptr), v(d_sq_dist_ptr)))
+
+    def knn(self, xyz, k, sq_radius=np.inf, T=None, exclude=None, stats=False):
+        """-> (index [n, k] int32, sq_dist [n, k] float32): for every query point x the k resident P points nearest to T x
+        (x when T is None) with d^2 <= sq_radius and index != exclude, in ascending (d^2, index); a row with fewer is padded
+        with -1 / +inf.  1 <= k <= 64; see s4g.h.  stats=True: also {P points tested, coarse blocks scanned} summed over
+        the queries."""
+        xyz = _c(xyz).reshape(-1, 3)
+        n, k = len(xyz), int(k)
+        T = None if T is None else _c(T).reshape(16)
+        exclude = None if exclude is None else _c(exclude, np.int32).reshape(n)
+        index, sq = np.empty((n, max(k, 0)), np.int32), np.empty((n, max(k, 0)), _f)
+        if not stats:
+            self._chk(self._L.s4g_knn(self.h, _p(xyz), n, _p(T), k, float(sq_radius), _p(exclude), _p(index), _p(sq)))
+            return index, sq
+        out = np.zeros(2, np.uint64)
+        self._chk(self._L.s4g_knn_probe_stats(self.h, _p(xyz), n, _p(T), k, float(sq_radius), _p(exclude), _p(index),
+                                              _p(sq), _p(out)))
+        return index, sq, dict(tested=int(out[0]), blocks=int(out[1]))
+
+    def knn_dev(self, d_xyz_ptr, n, k, d_index_ptr, d_sq_dist_ptr=None, sq_radius=np.inf, d_T_ptr=None, d_exclude_ptr=None):
+        """device pointers (n x 3 float32 queries, n x k int32 / float32 results, 16 float32 T, n int32 exclude; the last
+        three may be None), stream-ordered, nothing synchronised"""
+        v = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        self._chk(self._L.s4g_knn_dev(self.h, v(d_xyz_ptr), int(n), v(d_T_ptr), int(k), float(sq_radius), v(d_exclude_ptr),
+                                      v(d_index_ptr), v(d_sq_dist_ptr)))
 
     def range_query(self, xyz, sq_radius, T=None):
         """-> (offsets [n + 1] int64, indices [total] int32, sq_dist [total] float32): for every query point x, every
