@@ -1,0 +1,63 @@
+// super4pcs-b200: Utils::EstimateNormals on top of s4g_normals (include/s4g.h).
+#include "super4pcs/utils/normals.h"
+
+#include <algorithm>
+#include <cmath>
+#include <cstdlib>
+#include <stdexcept>
+#include <string>
+
+#include "s4g.h"
+
+namespace GlobalRegistration {
+namespace Utils {
+
+namespace {
+// the grid's delta of a cloud: 0.5 * E * sqrt(k / n), E the largest edge of its bounding box; 1 when E is 0
+float GridDelta(const std::vector<float>& xyz, std::size_t n, int k) {
+  float lo[3] = {xyz[0], xyz[1], xyz[2]}, hi[3] = {xyz[0], xyz[1], xyz[2]};
+  for (std::size_t i = 0; i < n; ++i)
+    for (int c = 0; c < 3; ++c) {
+      lo[c] = std::min(lo[c], xyz[3 * i + c]);
+      hi[c] = std::max(hi[c], xyz[3 * i + c]);
+    }
+  const double E = std::max({double(hi[0]) - lo[0], double(hi[1]) - lo[1], double(hi[2]) - lo[2]});
+  const float delta = float(0.5 * E * std::sqrt(double(k) / double(n)));
+  return delta > 0.f ? delta : 1.f;
+}
+}  // namespace
+
+int EstimateNormals(std::vector<Point3D>& cloud, int k, Point3D::Scalar max_distance,
+                    const Point3D::VectorType* viewpoint) {
+  if (std::isnan(max_distance) || max_distance < 0)
+    throw std::runtime_error("super4pcs-b200: EstimateNormals: max_distance is negative or NaN");
+  if (cloud.empty()) return 0;
+  const std::size_t n = cloud.size();
+  std::vector<float> xyz(3 * n);
+  for (std::size_t i = 0; i < n; ++i)
+    for (int c = 0; c < 3; ++c) xyz[3 * i + c] = cloud[i].pos()[c];
+  int device = 0;
+  if (const char* e = std::getenv("S4PCS_DEVICE")) device = std::atoi(e);
+  s4g_ctx* ctx = nullptr;
+  if (s4g_create(device, &ctx) != S4G_OK)
+    throw std::runtime_error("super4pcs-b200: EstimateNormals: no CUDA device (there is no CPU fallback)");
+  std::vector<float> normals(3 * n);
+  const float vp[3] = {viewpoint ? (*viewpoint)[0] : 0.f, viewpoint ? (*viewpoint)[1] : 0.f,
+                       viewpoint ? (*viewpoint)[2] : 0.f};
+  int rc = s4g_set_cloud_p(ctx, xyz.data(), int(n), GridDelta(xyz, n, k));
+  if (rc == S4G_OK)
+    rc = s4g_normals(ctx, k, max_distance * max_distance, viewpoint ? vp : nullptr, normals.data(), nullptr);
+  const std::string msg = rc == S4G_OK ? std::string() : std::string(s4g_error_string(ctx));
+  s4g_destroy(ctx);
+  if (rc != S4G_OK) throw std::runtime_error("super4pcs-b200: EstimateNormals: " + msg);
+  int nonzero = 0;
+  for (std::size_t i = 0; i < n; ++i) {
+    const Point3D::VectorType v(normals[3 * i], normals[3 * i + 1], normals[3 * i + 2]);
+    cloud[i].set_normal(v);
+    nonzero += v.squaredNorm() > 0.f ? 1 : 0;
+  }
+  return nonzero;
+}
+
+}  // namespace Utils
+}  // namespace GlobalRegistration

@@ -145,6 +145,28 @@ int s4g_knn_dev(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T_colmaj
                 const int32_t* d_exclude, int32_t* d_index, float* d_sq_dist);
 int s4g_knn_probe_stats(s4g_ctx* ctx, const float* xyz, int n, const float* T_colmajor, int k, float sq_radius,
                         const int32_t* exclude, int32_t* index, float* sq_dist, uint64_t* out2);
+/* Normals of the resident sampled P by PCA of k-nearest neighbourhoods, for every point j in the order of the array passed
+ * to s4g_set_cloud_p: normals[3j .. 3j+3), eigenvalues[3j .. 3j+3).
+ *   Neighbourhood: exactly the s4g_knn row of the query p_j (no T, no exclusion, the same k and sq_radius), so p_j itself
+ *   is in it unless more than k points coincide with it; the padding is skipped; m >= 1 real entries.
+ *   Arithmetic, all in double, sums from 0 in row order (ascending (d^2, j)): c = sum p / m, C = sum (p - c)(p - c)^T / m,
+ *   then cyclic Jacobi rotations on C (pairs (0,1), (0,2), (1,2) per sweep; an off-diagonal entry is zeroed when 100 |a_pq|
+ *   is lost against both |a_pp| and |a_qq|) until the off-diagonal is exactly zero, at most 50 sweeps.  Only + - * /,
+ *   sqrt and comparisons: a CPU restatement with no FMA gives the same bits.
+ *   eigenvalues = lambda0 <= lambda1 <= lambda2, the diagonal sorted stably (equal values keep the order of the Jacobi
+ *   columns, which start as the x, y, z axes), rounded to float.  Curvature is lambda0 / (lambda0 + lambda1 + lambda2).
+ *   normal = the Jacobi column of lambda0 (ties: the first of the equal columns in that order), normalised in double,
+ *   rounded to float.  Sign: with a viewpoint v (3 floats), negated when (v - p_j) . n < 0 in double; with viewpoint NULL,
+ *   the returned float normal's component of largest magnitude is made positive, ties to the lowest axis.
+ *   No normal: m < 3 or C exactly zero (e.g. coincident points) -> (0, 0, 0), which the pair filter skips; the
+ *   eigenvalues are written all the same.
+ * 3 <= k <= 64, sq_radius >= 0 and not NaN (+inf = unbounded), normals != NULL; otherwise S4G_ERR_ARG.  Needs
+ * s4g_set_cloud_p (S4G_ERR_STATE before it); scratch the device cannot hold (nP x (k + 3) 4-byte words) -> S4G_ERR_NOMEM.
+ * eigenvalues may be NULL.
+ * _dev: device buffers (nP x 3 floats each), enqueued on the context's stream, nothing synchronised; viewpoint is 3 host
+ * floats (or NULL), read before the call returns.                                                                      */
+int s4g_normals(s4g_ctx* ctx, int k, float sq_radius, const float* viewpoint, float* normals, float* eigenvalues);
+int s4g_normals_dev(s4g_ctx* ctx, int k, float sq_radius, const float* viewpoint, float* d_normals, float* d_eigenvalues);
 /* The range query of the reference's kd-tree (KdTree::doQueryDist / doQueryDistIndices / doQueryDistProcessIndices,
  * accelerators/kdtree.h:231-262, body :462-514) on the resident sampled P, for n arbitrary query points xyz (n x 3):
  * the list of query i is every j with d^2 = |y_i - p_j|^2 < sq_radius (strict, the kd-tree's point test kdtree.h:485),

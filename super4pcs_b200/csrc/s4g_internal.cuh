@@ -357,3 +357,8 @@ __device__ __forceinline__ void s4g_verify_record(const float (&m)[12], const Ve
 // Enqueue Verify of K candidate records (device); zeroes d_counts first.  d_K: the candidate count when only the device
 // knows it (K is then its upper bound)
 int s4g_launch_verify(s4g_ctx* ctx, const VerifyCand* d_recs, int K, uint32_t* d_counts, bool timed, const uint32_t* d_K);
+// Enqueue the k_knn instance of k (1 <= k <= 64) on the context's stream: the rows of s4g_knn_dev for n device queries
+// (verify.cu).  The arguments are checked by the caller, and n > 0.  stats: nullptr or the two counters of the statistics
+// variant.
+int s4g_launch_knn(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T, int k, float sq_radius,
+                   const int32_t* d_exclude, int32_t* d_index, float* d_sq_dist, unsigned long long* stats);

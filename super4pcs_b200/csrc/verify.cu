@@ -1413,8 +1413,8 @@ static void launch_knn_cap(s4g_ctx* ctx, unsigned nblk, const float* d_xyz, int 
                                                            d_sq_dist, nullptr);
 }
 
-static int launch_knn(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T, int k, float sq_radius,
-                      const int32_t* d_exclude, int32_t* d_index, float* d_sq_dist, unsigned long long* stats) {
+int s4g_launch_knn(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T, int k, float sq_radius,
+                   const int32_t* d_exclude, int32_t* d_index, float* d_sq_dist, unsigned long long* stats) {
   S4G_CUDA(cudaSetDevice(ctx->device));
   const unsigned nblk = (unsigned)((n + kThreads - 1) / kThreads);
   if (k <= 8)
@@ -1435,7 +1435,7 @@ extern "C" int s4g_knn_dev(s4g_ctx* ctx, const float* d_xyz, int n, const float*
   if (!ctx) return S4G_ERR_ARG;
   S4G_TRY(knn_args(ctx, "s4g_knn_dev", n, d_xyz, k, sq_radius, d_index));
   if (n == 0) return S4G_OK;
-  return launch_knn(ctx, d_xyz, n, d_T, k, sq_radius, d_exclude, d_index, d_sq_dist, nullptr);
+  return s4g_launch_knn(ctx, d_xyz, n, d_T, k, sq_radius, d_exclude, d_index, d_sq_dist, nullptr);
 }
 
 static int knn_host(s4g_ctx* ctx, const char* who, const float* xyz, int n, const float* T, int k, float sq_radius,
@@ -1446,7 +1446,7 @@ static int knn_host(s4g_ctx* ctx, const char* who, const float* xyz, int n, cons
   return query_host(ctx, xyz, n, T, k, exclude, index, sq_dist, stats,
                     [&](const float* d_xyz, const float* d_T, const int32_t* d_excl, int32_t* d_index, float* d_sq,
                         unsigned long long* d_stats) {
-                      return launch_knn(ctx, d_xyz, n, d_T, k, sq_radius, d_excl, d_index, d_sq, d_stats);
+                      return s4g_launch_knn(ctx, d_xyz, n, d_T, k, sq_radius, d_excl, d_index, d_sq, d_stats);
                     });
 }
 

@@ -99,6 +99,8 @@ def load_library():
         "s4g_knn": ([vp, vp, i32, vp, i32, f32, vp, vp, vp], i32),
         "s4g_knn_dev": ([vp, vp, i32, vp, i32, f32, vp, vp, vp], i32),
         "s4g_knn_probe_stats": ([vp, vp, i32, vp, i32, f32, vp, vp, vp, vp], i32),
+        "s4g_normals": ([vp, i32, f32, vp, vp, vp], i32),
+        "s4g_normals_dev": ([vp, i32, f32, vp, vp, vp], i32),
         "s4g_range": ([vp, vp, i32, vp, f32, vp, vp], i32),
         "s4g_get_range": ([vp, vp, vp], i32),
         "s4g_range_count_dev": ([vp, vp, i32, vp, f32, vp], i32),
@@ -319,6 +321,26 @@ class Context:
         v = lambda p: C.c_void_p(p) if p else None  # noqa: E731
         self._chk(self._L.s4g_knn_dev(self.h, v(d_xyz_ptr), int(n), v(d_T_ptr), int(k), float(sq_radius), v(d_exclude_ptr),
                                       v(d_index_ptr), v(d_sq_dist_ptr)))
+
+    def normals(self, k, sq_radius=np.inf, viewpoint=None):
+        """-> (normals [nP, 3] float32, eigenvalues [nP, 3] float32): for every resident P point, in the order of
+        set_cloud_p, the PCA normal of its k-nearest row (s4g_knn of the point itself within sq_radius) and the
+        covariance's eigenvalues, ascending.  Unoriented normals have their largest component positive; with a viewpoint
+        (3 floats) they face it.  (0, 0, 0) where the row holds fewer than 3 points or they coincide.  3 <= k <= 64; see
+        s4g.h."""
+        n = self.nP
+        vp = None if viewpoint is None else _c(viewpoint).reshape(3)
+        normals, eig = np.empty((n, 3), _f), np.empty((n, 3), _f)
+        self._chk(self._L.s4g_normals(self.h, int(k), float(sq_radius), _p(vp), _p(normals), _p(eig)))
+        return normals, eig
+
+    def normals_dev(self, k, d_normals_ptr, d_eigenvalues_ptr=None, sq_radius=np.inf, viewpoint=None):
+        """device pointers (nP x 3 float32 normals; nP x 3 float32 eigenvalues or None), stream-ordered, nothing
+        synchronised; viewpoint: 3 floats or None, as in normals"""
+        v = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        vp = None if viewpoint is None else _c(viewpoint).reshape(3)
+        self._chk(self._L.s4g_normals_dev(self.h, int(k), float(sq_radius), _p(vp), v(d_normals_ptr),
+                                          v(d_eigenvalues_ptr)))
 
     def range_query(self, xyz, sq_radius, T=None):
         """-> (offsets [n + 1] int64, indices [total] int32, sq_dist [total] float32): for every query point x, every
