@@ -7,25 +7,11 @@
 #include <stdexcept>
 #include <string>
 
+#include "grid_delta.h"
 #include "s4g.h"
 
 namespace GlobalRegistration {
 namespace Utils {
-
-namespace {
-// the grid's delta of a cloud: 0.5 * E * sqrt(k / n), E the largest edge of its bounding box; 1 when E is 0
-float GridDelta(const std::vector<float>& xyz, std::size_t n, int k) {
-  float lo[3] = {xyz[0], xyz[1], xyz[2]}, hi[3] = {xyz[0], xyz[1], xyz[2]};
-  for (std::size_t i = 0; i < n; ++i)
-    for (int c = 0; c < 3; ++c) {
-      lo[c] = std::min(lo[c], xyz[3 * i + c]);
-      hi[c] = std::max(hi[c], xyz[3 * i + c]);
-    }
-  const double E = std::max({double(hi[0]) - lo[0], double(hi[1]) - lo[1], double(hi[2]) - lo[2]});
-  const float delta = float(0.5 * E * std::sqrt(double(k) / double(n)));
-  return delta > 0.f ? delta : 1.f;
-}
-}  // namespace
 
 int EstimateNormals(std::vector<Point3D>& cloud, int k, Point3D::Scalar max_distance,
                     const Point3D::VectorType* viewpoint) {
@@ -44,7 +30,7 @@ int EstimateNormals(std::vector<Point3D>& cloud, int k, Point3D::Scalar max_dist
   std::vector<float> normals(3 * n);
   const float vp[3] = {viewpoint ? (*viewpoint)[0] : 0.f, viewpoint ? (*viewpoint)[1] : 0.f,
                        viewpoint ? (*viewpoint)[2] : 0.f};
-  int rc = s4g_set_cloud_p(ctx, xyz.data(), int(n), GridDelta(xyz, n, k));
+  int rc = s4g_set_cloud_p(ctx, xyz.data(), int(n), internal::GridDelta(xyz, n, k));
   if (rc == S4G_OK)
     rc = s4g_normals(ctx, k, max_distance * max_distance, viewpoint ? vp : nullptr, normals.data(), nullptr);
   const std::string msg = rc == S4G_OK ? std::string() : std::string(s4g_error_string(ctx));

@@ -167,6 +167,39 @@ int s4g_knn_probe_stats(s4g_ctx* ctx, const float* xyz, int n, const float* T_co
  * floats (or NULL), read before the call returns.                                                                      */
 int s4g_normals(s4g_ctx* ctx, int k, float sq_radius, const float* viewpoint, float* normals, float* eigenvalues);
 int s4g_normals_dev(s4g_ctx* ctx, int k, float sq_radius, const float* viewpoint, float* d_normals, float* d_eigenvalues);
+/* Outlier removal on the resident sampled P.  j is the position in the array passed to s4g_set_cloud_p.  Both filters
+ * write the kept j in ascending order to keep[0 .. *n_kept) (capacity nP; the output form of s4g_voxel_sample).
+ *
+ * Statistical filter (PCL's StatisticalOutlierRemoval, made exact):
+ *   Row of j: exactly the s4g_knn row of the query p_j with exclude = j, no T, sq_radius = +inf: m = min(k, nP - 1) real
+ *   entries, d2_e the floats s4g_knn returns.
+ *   mean_dist[j] = (sum over the row in row order, from 0.0, of sqrt((double) d2_e)) / m.
+ *   mu and sigma in double, each sum in this fixed order: the j in ascending order are cut into runs of 1024 (the last
+ *   may be shorter), each run summed left to right from 0.0, then the run sums left to right from 0.0.
+ *     mu = (sum of mean_dist) / nP;  sigma = sqrt((sum of (mean_dist - mu)^2) / (nP - 1)), a second pass in that order.
+ *   j is kept iff mean_dist[j] <= mu + std_ratio * sigma, in double.  Only + - * /, sqrt and comparisons, no FMA: a CPU
+ *   restatement compiled without contraction gives the same bits.  nP = 1: the point is kept, mean_dist = mu = sigma = 0.
+ *   out2 = {mu, sigma}.  mean_dist (nP doubles) and out2 may be NULL.
+ *   1 <= k <= 64 and std_ratio finite (any sign), keep and n_kept != NULL; otherwise S4G_ERR_ARG.  Needs s4g_set_cloud_p
+ *   (S4G_ERR_STATE before it); scratch the device cannot hold (about nP x (2k + 6) 4-byte words) -> S4G_ERR_NOMEM.
+ *
+ * Radius filter (PCL's RadiusOutlierRemoval, made exact):
+ *   c_j = #{i != j : d^2(p_i, p_j) < sq_radius}, d^2 and the strict test exactly as in s4g_range: for sq_radius > 0, c_j
+ *   is the length of the s4g_range list of the query p_j minus 1 (p_j's own d^2 is exactly 0).  sq_radius <= 0: c_j = 0;
+ *   +inf: every other point with a finite d^2.
+ *   j is kept iff c_j >= min_neighbors.  counts[j] = min(c_j, min_neighbors): the count stops there (this is what makes
+ *   the filter cheap in dense regions), so the value is capped.  counts (nP int32) may be NULL.
+ *   sq_radius not NaN, min_neighbors >= 1, keep and n_kept != NULL; otherwise S4G_ERR_ARG.  STATE and NOMEM as above.
+ *
+ * _dev: device buffers (d_n_kept one int64), enqueued on the context's stream, nothing synchronised.                    */
+int s4g_statistical_outliers(s4g_ctx* ctx, int k, double std_ratio, int32_t* keep, int64_t* n_kept, double* mean_dist,
+                             double* out2);
+int s4g_statistical_outliers_dev(s4g_ctx* ctx, int k, double std_ratio, int32_t* d_keep, int64_t* d_n_kept,
+                                 double* d_mean_dist, double* d_out2);
+int s4g_radius_outliers(s4g_ctx* ctx, float sq_radius, int min_neighbors, int32_t* keep, int64_t* n_kept,
+                        int32_t* counts);
+int s4g_radius_outliers_dev(s4g_ctx* ctx, float sq_radius, int min_neighbors, int32_t* d_keep, int64_t* d_n_kept,
+                            int32_t* d_counts);
 /* The range query of the reference's kd-tree (KdTree::doQueryDist / doQueryDistIndices / doQueryDistProcessIndices,
  * accelerators/kdtree.h:231-262, body :462-514) on the resident sampled P, for n arbitrary query points xyz (n x 3):
  * the list of query i is every j with d^2 = |y_i - p_j|^2 < sq_radius (strict, the kd-tree's point test kdtree.h:485),

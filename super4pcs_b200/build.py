@@ -11,7 +11,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "lib", "obj")
 LIB = os.path.join(HERE, "lib", "libs4g.so")
-SOURCES = ["context.cu", "verify.cu", "rigid.cu", "pairs.cu", "quads.cu", "sampler.cu", "comm.cu", "normals.cu"]
+SOURCES = ["context.cu", "verify.cu", "rigid.cu", "pairs.cu", "quads.cu", "sampler.cu", "comm.cu", "normals.cu", "outliers.cu"]
 
 NVCC_FLAGS = [
     "-std=c++17", "-O3",

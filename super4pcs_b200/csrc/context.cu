@@ -133,7 +133,7 @@ extern "C" void s4g_destroy(s4g_ctx* ctx) {
                    &ctx->dMisc, &ctx->bArgs, &ctx->bCounts, &ctx->bPairKeys[0], &ctx->bPairKeys[1], &ctx->bQKeys[0], &ctx->bQKeys[1],
                    &ctx->bQVals[0], &ctx->bQVals[1], &ctx->bQCnt, &ctx->bQuadKeys[0], &ctx->bQuadKeys[1], &ctx->bQuads, &ctx->bMisc,
                    &ctx->bResults, &ctx->dQpatch, &ctx->dVrec, &ctx->dVsort, &ctx->dRangeOff, &ctx->dRangeIdx,
-                   &ctx->dRangeSq};
+                   &ctx->dRangeSq, &ctx->dFilter};
   for (DevBuf* b : all) free_buf(ctx, *b);
   cudaStreamSynchronize(ctx->stream);
   if (ctx->hPinned) cudaFreeHost(ctx->hPinned);

@@ -189,9 +189,7 @@ int launch_normals(s4g_ctx* ctx, int k, float sq_radius, const float* viewpoint,
   S4G_TRY(s4g_reserve(ctx, ctx->dScratchB, (size_t)n * (size_t)k * sizeof(int32_t)));
   float* d_xyz = ctx->dScratchA.as<float>();
   int32_t* d_rows = ctx->dScratchB.as<int32_t>();
-  k_normals_queries<<<nblk(n, 256), 256, 0, ctx->stream>>>(ctx->grid.pts, n, d_xyz);
-  ctx->launches++;
-  S4G_CUDA(cudaGetLastError());
+  S4G_TRY(s4g_launch_sorted_queries(ctx, d_xyz));
   S4G_TRY(s4g_launch_knn(ctx, d_xyz, n, nullptr, k, sq_radius, nullptr, d_rows, nullptr, nullptr));
   const bool has_vp = viewpoint != nullptr;
   k_normals<<<nblk(n, kNormalsThreads), kNormalsThreads, 0, ctx->stream>>>(
@@ -203,6 +201,14 @@ int launch_normals(s4g_ctx* ctx, int k, float sq_radius, const float* viewpoint,
 }
 
 }  // namespace
+
+int s4g_launch_sorted_queries(s4g_ctx* ctx, float* d_xyz) {
+  S4G_CUDA(cudaSetDevice(ctx->device));
+  k_normals_queries<<<nblk(ctx->nP, 256), 256, 0, ctx->stream>>>(ctx->grid.pts, ctx->nP, d_xyz);
+  ctx->launches++;
+  S4G_CUDA(cudaGetLastError());
+  return S4G_OK;
+}
 
 extern "C" int s4g_normals_dev(s4g_ctx* ctx, int k, float sq_radius, const float* viewpoint, float* d_normals,
                                float* d_eigenvalues) {

@@ -212,6 +212,7 @@ struct s4g_ctx {
   DevBuf dScratchA, dScratchB, dScratchC, dScratchD, dCub;
   DevBuf dRms, dOk, dCandIdx, dCounts, dResult, dMisc;
   DevBuf dVrec, dVsort;   // Verify: per-candidate records; per-patch candidate order (sort keys, values, CUB temp)
+  DevBuf dFilter;         // the outlier filters' host forms: their device outputs before the copy back (outliers.cu)
   void* hPinned = nullptr;  // small pinned staging block
   size_t hPinnedBytes = 0;
 
@@ -362,3 +363,8 @@ int s4g_launch_verify(s4g_ctx* ctx, const VerifyCand* d_recs, int K, uint32_t* d
 // variant.
 int s4g_launch_knn(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T, int k, float sq_radius,
                    const int32_t* d_exclude, int32_t* d_index, float* d_sq_dist, unsigned long long* stats);
+// Enqueue the resident P points in the grid's sorted order as n x 3 queries (normals.cu): query t is GridDev::pts[t]
+int s4g_launch_sorted_queries(s4g_ctx* ctx, float* d_xyz);
+// Enqueue k_radius_count over the resident P (verify.cu): d_counts[j] = min(c_j, min_neighbors) (d_counts may be
+// nullptr), d_keep[j] = c_j >= min_neighbors, c_j the number of other P points with d^2 < sq_radius.  min_neighbors >= 1.
+int s4g_launch_radius_count(s4g_ctx* ctx, float sq_radius, int min_neighbors, int32_t* d_counts, uint8_t* d_keep);

@@ -873,6 +873,106 @@ k_range(GridDev g, const float* __restrict__ xyz, int n, const float* __restrict
   if (!kFill) offsets[i] = out;
 }
 
+// ---- the neighbour counts of the radius outlier filter (s4g_radius_outliers): for every resident P point j,
+// c_j = #{i != j : d^2(p_i, p_j) < sq_radius}, counted up to min_neighbors.  One thread per sorted point t (GridDev::pts,
+// w = original index j); the query is p_j as stored, d^2 as in k_range.
+//
+// Search.  k_range's descent and point test with the bound sq_radius: a box, or a cell row of a block, is dropped when csat
+// says it is empty or when cells_bound(...) >= sq_radius, and a point is counted when d^2 < sq_radius and its index is not
+// j.  Run to the end, that count is k_range's list of p_j without j's own entry (its d^2 to itself is exactly 0, in the list
+// whenever sq_radius > 0) -- exact by k_range's argument, whatever the order of the descent.  The thread stops as soon as
+// the count reaches min_neighbors: every point adds at most 1, so it stops at min(c_j, min_neighbors) in any search
+// order, and that capped value is all the filter needs.  In a dense region a thread opens a few cells however loose the
+// radius; without the cap it would cost what k_range's count pass costs.  sq_radius <= 0 drops the root (c_j = 0).
+// counts[j] = the capped count (counts may be nullptr); keep[j] = 1 when it reached min_neighbors, else 0.
+__global__ void __launch_bounds__(kThreads)
+k_radius_count(GridDev g, int n, float sq_radius, int min_neighbors, int32_t* __restrict__ counts,
+               uint8_t* __restrict__ keep) {
+  const long long t = (long long)blockIdx.x * kThreads + threadIdx.x;
+  if (t >= n) return;
+  const float4 self = __ldg(&g.pts[t]);
+  NearestQuery q;
+  q.tx = self.x;
+  q.ty = self.y;
+  q.tz = self.z;
+  q.excl = __float_as_int(self.w);
+  int c = 0;
+  const double ih = (double)g.inv_h;
+  q.ux = ((double)q.tx - (double)g.ox) * ih;
+  q.uy = ((double)q.ty - (double)g.oy) * ih;
+  q.uz = ((double)q.tz - (double)g.oz) * ih;
+  q.eps = (double)(max(g.nx, max(g.ny, g.nz)) + 2) * 0x1p-21;
+  q.h2 = 1.0 / (ih * ih);
+  const int cs = g.cshift, mx = g.nx - 1, my = g.ny - 1, mz = g.nz - 1;
+  const BrickShape bs = brick_shape(g);
+  BlockBox stack[kNearestStack];
+  int top = 0;
+  stack[top++] = BlockBox{box_axis(0, g.cnx - 1), box_axis(0, g.cny - 1), box_axis(0, g.cnz - 1)};
+#pragma unroll 1
+  while (top > 0 && c < min_neighbors) {
+    const BlockBox b = stack[--top];
+    const int x0 = box_lo(b.x), x1 = box_hi(b.x), y0 = box_lo(b.y), y1 = box_hi(b.y), z0 = box_lo(b.z), z1 = box_hi(b.z);
+    const int cx0 = x0 << cs, cy0 = y0 << cs, cz0 = z0 << cs;
+    const int cx1 = min(((x1 + 1) << cs) - 1, mx), cy1 = min(((y1 + 1) << cs) - 1, my), cz1 = min(((z1 + 1) << cs) - 1, mz);
+    if (cx0 > cx1 || cy0 > cy1 || cz0 > cz1) continue;
+    if (cells_bound(q, cx0, cx1, cy0, cy1, cz0, cz1) >= sq_radius) continue;
+    if (csat_count(g, x0, x1, y0, y1, z0, z1) == 0u) continue;
+    const int ex = x1 - x0, ey = y1 - y0, ez = z1 - z0;
+    if ((ex | ey | ez) != 0) {                       // halve the longest axis, the nearer half searched first
+      BlockBox lo = b, hi = b;
+      bool lo_near;
+      if (ex >= ey && ex >= ez) {
+        const int mid = (x0 + x1) >> 1;
+        lo.x = box_axis(x0, mid);
+        hi.x = box_axis(mid + 1, x1);
+        lo_near = q.ux < (double)((mid + 1) << cs);
+      } else if (ey >= ez) {
+        const int mid = (y0 + y1) >> 1;
+        lo.y = box_axis(y0, mid);
+        hi.y = box_axis(mid + 1, y1);
+        lo_near = q.uy < (double)((mid + 1) << cs);
+      } else {
+        const int mid = (z0 + z1) >> 1;
+        lo.z = box_axis(z0, mid);
+        hi.z = box_axis(mid + 1, z1);
+        lo_near = q.uz < (double)((mid + 1) << cs);
+      }
+      stack[top++] = lo_near ? hi : lo;
+      stack[top++] = lo_near ? lo : hi;
+      continue;
+    }
+    // one block: its cell rows within the bound, one contiguous run of sorted points per brick a row crosses
+#pragma unroll 1
+    for (int cz = cz0; cz <= cz1; ++cz)
+#pragma unroll 1
+      for (int cy = cy0; cy <= cy1; ++cy) {
+        if (cells_bound(q, cx0, cx1, cy, cy, cz, cz) >= sq_radius) continue;
+        const int rowb = brick_row(g, bs, cy, cz);
+        const uint32_t rowl = cell_row(bs, cy, cz);
+#pragma unroll 1
+        for (int cx = cx0; cx <= cx1;) {
+          const int xe = min(cx1, cx | bs.m);
+          const int rank = __ldg(&g.top[brick_in_row(bs, rowb, cx)]);
+          if (rank >= 0) {
+            const uint32_t s = __ldg(&g.cellStart[cell_in_row(bs, rank, rowl, cx)]);
+            const uint32_t e = __ldg(&g.cellStart[cell_in_row(bs, rank, rowl, xe) + 1u]);
+#pragma unroll 1
+            for (uint32_t k = s; k < e; ++k) {
+              const float4 p = __ldg(&g.pts[k]);
+              const float dx = __fsub_rn(q.tx, p.x), dy = __fsub_rn(q.ty, p.y), dz = __fsub_rn(q.tz, p.z);
+              const float d2 = __fadd_rn(__fmul_rn(dx, dx), __fadd_rn(__fmul_rn(dy, dy), __fmul_rn(dz, dz)));
+              if (d2 < sq_radius && __float_as_int(p.w) != q.excl && ++c == min_neighbors) goto done;
+            }
+          }
+          cx = xe + 1;
+        }
+      }
+  }
+done:
+  if (counts != nullptr) counts[q.excl] = c;
+  keep[q.excl] = c >= min_neighbors ? 1 : 0;
+}
+
 // the segments of one sort chunk (s4g_range): query i's list is [offsets[i], offsets[i + 1]); the chunk takes the lists
 // that start in [base, base + window), relative to base, and gives every other query an empty segment
 __global__ void k_range_chunk(const int64_t* __restrict__ offsets, int n, int64_t base, int64_t window,
@@ -1460,6 +1560,16 @@ extern "C" int s4g_knn_probe_stats(s4g_ctx* ctx, const float* xyz, int n, const 
   if (ctx && !out2) { ctx->err = "s4g_knn_probe_stats: bad arguments"; return S4G_ERR_ARG; }
   if (out2) out2[0] = out2[1] = 0;
   return knn_host(ctx, "s4g_knn_probe_stats", xyz, n, T, k, sq_radius, exclude, index, sq_dist, out2);
+}
+
+int s4g_launch_radius_count(s4g_ctx* ctx, float sq_radius, int min_neighbors, int32_t* d_counts, uint8_t* d_keep) {
+  S4G_CUDA(cudaSetDevice(ctx->device));
+  const int n = ctx->nP;
+  k_radius_count<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, 0, ctx->stream>>>(ctx->grid, n, sq_radius,
+                                                                                          min_neighbors, d_counts, d_keep);
+  ctx->launches++;
+  S4G_CUDA(cudaGetLastError());
+  return S4G_OK;
 }
 
 static int range_args(s4g_ctx* ctx, const char* who, int n, const void* xyz, float sq_radius, const void* offsets) {

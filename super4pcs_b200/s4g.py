@@ -101,6 +101,10 @@ def load_library():
         "s4g_knn_probe_stats": ([vp, vp, i32, vp, i32, f32, vp, vp, vp, vp], i32),
         "s4g_normals": ([vp, i32, f32, vp, vp, vp], i32),
         "s4g_normals_dev": ([vp, i32, f32, vp, vp, vp], i32),
+        "s4g_statistical_outliers": ([vp, i32, C.c_double, vp, vp, vp, vp], i32),
+        "s4g_statistical_outliers_dev": ([vp, i32, C.c_double, vp, vp, vp, vp], i32),
+        "s4g_radius_outliers": ([vp, f32, i32, vp, vp, vp], i32),
+        "s4g_radius_outliers_dev": ([vp, f32, i32, vp, vp, vp], i32),
         "s4g_range": ([vp, vp, i32, vp, f32, vp, vp], i32),
         "s4g_get_range": ([vp, vp, vp], i32),
         "s4g_range_count_dev": ([vp, vp, i32, vp, f32, vp], i32),
@@ -341,6 +345,41 @@ class Context:
         vp = None if viewpoint is None else _c(viewpoint).reshape(3)
         self._chk(self._L.s4g_normals_dev(self.h, int(k), float(sq_radius), _p(vp), v(d_normals_ptr),
                                           v(d_eigenvalues_ptr)))
+
+    def statistical_outliers(self, k, std_ratio):
+        """-> (keep [n_kept] int32, mean_dist [nP] float64, mu, sigma): the resident P points (positions in the array of
+        set_cloud_p, ascending) whose mean distance to their k nearest other points is at most mu + std_ratio * sigma, mu
+        and sigma the mean and sample standard deviation of those means over P.  1 <= k <= 64; see s4g.h."""
+        n = self.nP
+        keep, mean, out2 = np.empty(n, np.int32), np.empty(n, np.float64), np.zeros(2, np.float64)
+        nk = C.c_int64(0)
+        self._chk(self._L.s4g_statistical_outliers(self.h, int(k), float(std_ratio), _p(keep), C.byref(nk), _p(mean),
+                                                   _p(out2)))
+        return keep[:nk.value].copy(), mean, float(out2[0]), float(out2[1])
+
+    def statistical_outliers_dev(self, k, std_ratio, d_keep_ptr, d_n_kept_ptr, d_mean_dist_ptr=None, d_out2_ptr=None):
+        """device pointers (nP int32 keep, 1 int64 n_kept, nP float64 mean_dist or None, 2 float64 {mu, sigma} or None),
+        stream-ordered, nothing synchronised"""
+        v = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        self._chk(self._L.s4g_statistical_outliers_dev(self.h, int(k), float(std_ratio), v(d_keep_ptr), v(d_n_kept_ptr),
+                                                       v(d_mean_dist_ptr), v(d_out2_ptr)))
+
+    def radius_outliers(self, sq_radius, min_neighbors):
+        """-> (keep [n_kept] int32, counts [nP] int32): the resident P points (ascending positions) with at least
+        min_neighbors other P points at d^2 < sq_radius; counts[j] = that number, capped at min_neighbors.  See s4g.h."""
+        n = self.nP
+        keep, counts = np.empty(n, np.int32), np.empty(n, np.int32)
+        nk = C.c_int64(0)
+        self._chk(self._L.s4g_radius_outliers(self.h, float(sq_radius), int(min_neighbors), _p(keep), C.byref(nk),
+                                              _p(counts)))
+        return keep[:nk.value].copy(), counts
+
+    def radius_outliers_dev(self, sq_radius, min_neighbors, d_keep_ptr, d_n_kept_ptr, d_counts_ptr=None):
+        """device pointers (nP int32 keep, 1 int64 n_kept, nP int32 counts or None), stream-ordered, nothing
+        synchronised"""
+        v = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        self._chk(self._L.s4g_radius_outliers_dev(self.h, float(sq_radius), int(min_neighbors), v(d_keep_ptr),
+                                                  v(d_n_kept_ptr), v(d_counts_ptr)))
 
     def range_query(self, xyz, sq_radius, T=None):
         """-> (offsets [n + 1] int64, indices [total] int32, sq_dist [total] float32): for every query point x, every
