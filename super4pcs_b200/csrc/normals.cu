@@ -2,7 +2,7 @@
 //
 // Rows.  The neighbourhood of P point j is exactly the s4g_knn row of the query p_j: no transform, no exclusion, the
 // caller's k and sq_radius.  It holds p_j itself unless more than k points coincide with it.  The rows come from the
-// existing k_knn instances (verify.cu), fed the P points in the grid's sorted order (GridDev::pts, w = original index)
+// existing k_knn instances (query.cu), fed the P points in the grid's sorted order (GridDev::pts, w = original index)
 // so that neighbouring threads descend neighbouring boxes; row t belongs to sorted point t.
 //
 // k_normals, one thread per sorted point t of original index j.  In double, over the m real entries of the row in row

@@ -2,7 +2,7 @@
 // the kept original indices j in ascending order and their number, compacted by cub::DeviceSelect::Flagged from a flag
 // per j (the output form of s4g_voxel_sample).
 //
-// Statistical filter.  Rows: the P points go to the existing k_knn instances (verify.cu) in the grid's sorted order
+// Statistical filter.  Rows: the P points go to the existing k_knn instances (query.cu) in the grid's sorted order
 // (s4g_launch_sorted_queries, as normals.cu), each excluding itself (exclude[t] = the original index of sorted point t),
 // no T, sq_radius = +inf.  So row t is the s4g_knn row of p_j with exclude = j: min(k, nP - 1) real entries.
 // k_outlier_mean, one thread per sorted point t of original index j: over the row's real entries in row order,
@@ -19,7 +19,7 @@
 // -fmad=false so that no product is contracted into an FMA.  A CPU restatement of the same operations compiled without
 // contraction (-ffp-contract=off) gives the same bits: mean_dist, mu, sigma and the kept set.
 //
-// Radius filter.  k_radius_count (verify.cu, next to k_range, whose descent and point test it shares) writes the capped
+// Radius filter.  k_radius_count (query.cu: the same descent, drop rule and point test as k_range) writes the capped
 // count and the flag of every j; its exactness argument is in its header.
 #include "s4g_internal.cuh"
 #include <cub/cub.cuh>

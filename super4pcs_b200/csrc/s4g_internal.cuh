@@ -311,6 +311,12 @@ __device__ __forceinline__ float3 s4_normalized(float3 a) {
   return a;
 }
 __device__ __forceinline__ float3 s4_xyz(float4 v) { return make_float3(v.x, v.y, v.z); }
+// T q in the reference's operation order: ((m0 x + m1 y) + m2 z) + m3 per row (Verify's exact test and the point queries)
+__device__ __forceinline__ void exact_tq(const float* __restrict__ m, float4 q, float& tx, float& ty, float& tz) {
+  tx = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[0], q.x), __fmul_rn(m[1], q.y)), __fmul_rn(m[2], q.z)), m[3]);
+  ty = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[4], q.x), __fmul_rn(m[5], q.y)), __fmul_rn(m[6], q.z)), m[7]);
+  tz = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(m[8], q.x), __fmul_rn(m[9], q.y)), __fmul_rn(m[10], q.z)), m[11]);
+}
 
 // ---- Verify's candidate records (verify.cu), written by whatever produces the candidates (k_pack_rec for the API
 // entry points, the rigid fits of rigid.cu), so that Verify needs no launch of its own to derive them
@@ -359,12 +365,12 @@ __device__ __forceinline__ void s4g_verify_record(const float (&m)[12], const Ve
 // knows it (K is then its upper bound)
 int s4g_launch_verify(s4g_ctx* ctx, const VerifyCand* d_recs, int K, uint32_t* d_counts, bool timed, const uint32_t* d_K);
 // Enqueue the k_knn instance of k (1 <= k <= 64) on the context's stream: the rows of s4g_knn_dev for n device queries
-// (verify.cu).  The arguments are checked by the caller, and n > 0.  stats: nullptr or the two counters of the statistics
+// (query.cu).  The arguments are checked by the caller, and n > 0.  stats: nullptr or the two counters of the statistics
 // variant.
 int s4g_launch_knn(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T, int k, float sq_radius,
                    const int32_t* d_exclude, int32_t* d_index, float* d_sq_dist, unsigned long long* stats);
 // Enqueue the resident P points in the grid's sorted order as n x 3 queries (normals.cu): query t is GridDev::pts[t]
 int s4g_launch_sorted_queries(s4g_ctx* ctx, float* d_xyz);
-// Enqueue k_radius_count over the resident P (verify.cu): d_counts[j] = min(c_j, min_neighbors) (d_counts may be
+// Enqueue k_radius_count over the resident P (query.cu): d_counts[j] = min(c_j, min_neighbors) (d_counts may be
 // nullptr), d_keep[j] = c_j >= min_neighbors, c_j the number of other P points with d^2 < sq_radius.  min_neighbors >= 1.
 int s4g_launch_radius_count(s4g_ctx* ctx, float sq_radius, int min_neighbors, int32_t* d_counts, uint8_t* d_keep);
