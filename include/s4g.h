@@ -200,6 +200,29 @@ int s4g_radius_outliers(s4g_ctx* ctx, float sq_radius, int min_neighbors, int32_
                         int32_t* counts);
 int s4g_radius_outliers_dev(s4g_ctx* ctx, float sq_radius, int min_neighbors, int32_t* d_keep, int64_t* d_n_kept,
                             int32_t* d_counts);
+/* Euclidean clusters of the resident sampled P (PCL's EuclideanClusterExtraction, made exact).  j is the position in the
+ * array passed to s4g_set_cloud_p.
+ *   Graph: an edge (i, j), i != j, iff d^2(p_i, p_j) < sq_radius, d^2 and the strict test exactly as in s4g_range (fp32,
+ *   dx^2 + (dy^2 + dz^2), no FMA).  The graph is symmetric bit for bit: under round to nearest fl(a - b) = -fl(b - a), so
+ *   d^2(p_i, p_j) and d^2(p_j, p_i) are the same float, and the search takes each edge once, from its larger end.
+ *   sq_radius <= 0: no edges; +inf: every pair with a finite d^2 (s4g_set_cloud_p refuses non-finite coordinates).
+ *   Components: root[j] = the smallest j' in j's connected component, before any size filter.
+ *   A component is a cluster iff min_size <= size <= max_size.  Clusters are ordered by size, descending, ties by root,
+ *   ascending (PCL sorts by size and leaves ties unspecified).  labels[j] = the rank of j's cluster in that order, -1 when
+ *   j's component is not a cluster; *n_clusters = their number.
+ *   Members in CSR form: cluster c is members[offsets[c] .. offsets[c + 1]), in ascending j.  Capacities nP + 1 (offsets)
+ *   and nP (members); only offsets[0 .. n_clusters] and members[0 .. offsets[n_clusters]) are defined.
+ *   Every output is integer work on the component partition, which depends on the edge set alone: the same bits on
+ *   every run.
+ * min_size >= 1 and max_size >= min_size (INT_MAX: no limit), sq_radius not NaN, labels and n_clusters != NULL;
+ * otherwise S4G_ERR_ARG.  root, offsets and members may be NULL.  Needs s4g_set_cloud_p (S4G_ERR_STATE before it);
+ * scratch the device cannot hold (24 bytes per P point, 44 in the host form, plus CUB's radix sort and scan storage)
+ * -> S4G_ERR_NOMEM.
+ * _dev: device buffers (d_n_clusters one int64), enqueued on the context's stream, nothing synchronised.             */
+int s4g_euclidean_clusters(s4g_ctx* ctx, float sq_radius, int min_size, int max_size, int32_t* labels, int32_t* root,
+                           int64_t* n_clusters, int64_t* offsets, int32_t* members);
+int s4g_euclidean_clusters_dev(s4g_ctx* ctx, float sq_radius, int min_size, int max_size, int32_t* d_labels,
+                               int32_t* d_root, int64_t* d_n_clusters, int64_t* d_offsets, int32_t* d_members);
 /* The range query of the reference's kd-tree (KdTree::doQueryDist / doQueryDistIndices / doQueryDistProcessIndices,
  * accelerators/kdtree.h:231-262, body :462-514) on the resident sampled P, for n arbitrary query points xyz (n x 3):
  * the list of query i is every j with d^2 = |y_i - p_j|^2 < sq_radius (strict, the kd-tree's point test kdtree.h:485),

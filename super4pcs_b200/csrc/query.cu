@@ -1,6 +1,7 @@
 // Point queries on the resident P grid, for arbitrary query points: the k nearest P points within a radius (s4g_knn;
-// s4g_nearest is its k = 1), every P point within a radius (s4g_range), and the capped neighbour counts of the radius
-// outlier filter (s4g_radius_outliers).  They are the reference kd-tree's queries: the restricted closest point
+// s4g_nearest is its k = 1), every P point within a radius (s4g_range), the capped neighbour counts of the radius
+// outlier filter (s4g_radius_outliers) and the union-find of the Euclidean clusters (s4g_euclidean_clusters).  They are
+// the reference kd-tree's queries: the restricted closest point
 // (KdTree::doQueryRestrictedClosestIndex, kdtree.h:388-453) and the range query (KdTree::doQueryDistProcessIndices,
 // kdtree.h:462-514).  One thread per query; y = T x (exact_tq) or x, and d^2 = dx^2 + (dy^2 + dz^2) in fp32 as in
 // Verify's exact test.
@@ -293,6 +294,120 @@ k_radius_count(GridDev g, int n, float sq_radius, int min_neighbors, int32_t* __
 done:
   if (counts != nullptr) counts[q.excl] = c;
   keep[q.excl] = c >= min_neighbors ? 1 : 0;
+}
+
+// ---- the union-find of the Euclidean clusters (s4g_euclidean_clusters, finished in clusters.cu): the graph on the
+// resident P with an edge (i, j), i != j, iff d^2(p_i, p_j) < sq_radius.  parent[] is indexed by original index and starts
+// as parent[x] = x; on return every edge's two endpoints are in one set, and sets were only ever joined along an edge.
+// One thread per
+// sorted point t (GridDev::pts, w = original index j); the query is p_j as stored, d^2 as in k_range.
+//
+// Search.  k_range's descent, drop rule and point test with the bound sq_radius: a box, or a cell row of a block, is
+// dropped when csat says it is empty or when cells_bound(...) >= sq_radius, and a point i is a neighbour when
+// d^2 < sq_radius.  Every neighbour i < j is merged with j (cluster_unite).  sq_radius <= 0 drops the root: no edges.
+// Invariant parent[x] <= x.  A hook writes parent[hi] = lo only where hi is a root (atomicCAS from hi) and lo < hi; the
+// path halving of cluster_find (s4g_internal.cuh) writes parent[x] = parent[parent[x]], an ancestor of x, so never above
+// x.  So parents strictly decrease along a path (no cycle), and the root of a set is its smallest index: the contract's
+// root, with no further reduction.  A node's ancestors only ever gain members of its own set, so a read that misses
+// another thread's write still returns an ancestor: it costs steps (or a failed atomicCAS), never a wrong merge.
+// Correctness.
+//   - Every edge is seen from its larger endpoint.  The descent is exact (the argument of the header and of k_range): the
+//     thread of j meets every i with d^2(p_j, p_i) < sq_radius.  The graph is symmetric bit for bit -- under round to
+//     nearest fl(a - b) = -fl(b - a), so each squared difference, and d^2, is the same float from either end -- so the
+//     edge (i, j), i < j, is met by j's thread, and taking only i < j loses none.
+//   - Concurrent hooks only merge sets that share an edge.  cluster_unite hooks a root only under a member of the other
+//     endpoint's set, found from that edge's two ends; a failed atomicCAS (the root was hooked meanwhile) retries from
+//     the new parent, and agreeing finds (both ends in one set, which stays so) end the call without a write.
+//   - So the final sets are the connected components: the result depends on the edge set only, not on thread order, and
+//     each component's root is its smallest index.
+// Registers.  __maxnreg__(64) stands in for __launch_bounds__ (the two exclude each other): left to itself, ptxas gives
+// this kernel 32 registers and spills in the point loop; at 64 it takes 60 and spills nothing.
+__device__ __forceinline__ void cluster_unite(int* parent, int a, int b) {
+#pragma unroll 1
+  while (true) {
+    const int ra = cluster_find(parent, a), rb = cluster_find(parent, b);
+    if (ra == rb) return;
+    const int hi = max(ra, rb), lo = min(ra, rb);
+    const int old = atomicCAS(&parent[hi], hi, lo);
+    if (old == hi) return;
+    a = old;   // hi was hooked meanwhile: retry from its new parent, in the same set
+    b = lo;
+  }
+}
+
+__global__ void __maxnreg__(64)
+k_cluster_link(GridDev g, int n, float sq_radius, int* __restrict__ parent) {
+  const long long t = (long long)blockIdx.x * kThreads + threadIdx.x;
+  if (t >= n) return;
+  const float4 self = __ldg(&g.pts[t]);
+  NearestQuery q;
+  q.tx = self.x;
+  q.ty = self.y;
+  q.tz = self.z;
+  q.excl = __float_as_int(self.w);
+  query_cells(g, q);
+  const int cs = g.cshift, mx = g.nx - 1, my = g.ny - 1, mz = g.nz - 1;
+  const BrickShape bs = brick_shape(g);
+  BlockBox stack[kNearestStack];
+  int top = 0;
+  stack[top++] = BlockBox{box_axis(0, g.cnx - 1), box_axis(0, g.cny - 1), box_axis(0, g.cnz - 1)};
+#pragma unroll 1
+  while (top > 0) {
+    const BlockBox b = stack[--top];
+    const int x0 = box_lo(b.x), x1 = box_hi(b.x), y0 = box_lo(b.y), y1 = box_hi(b.y), z0 = box_lo(b.z), z1 = box_hi(b.z);
+    const int cx0 = x0 << cs, cy0 = y0 << cs, cz0 = z0 << cs;
+    const int cx1 = min(((x1 + 1) << cs) - 1, mx), cy1 = min(((y1 + 1) << cs) - 1, my), cz1 = min(((z1 + 1) << cs) - 1, mz);
+    if (cx0 > cx1 || cy0 > cy1 || cz0 > cz1) continue;
+    if (cells_bound(q, cx0, cx1, cy0, cy1, cz0, cz1) >= sq_radius) continue;
+    if (csat_count(g, x0, x1, y0, y1, z0, z1) == 0u) continue;
+    const int ex = x1 - x0, ey = y1 - y0, ez = z1 - z0;
+    if ((ex | ey | ez) != 0) {                       // halve the longest axis
+      BlockBox lo = b, hi = b;
+      if (ex >= ey && ex >= ez) {
+        const int mid = (x0 + x1) >> 1;
+        lo.x = box_axis(x0, mid);
+        hi.x = box_axis(mid + 1, x1);
+      } else if (ey >= ez) {
+        const int mid = (y0 + y1) >> 1;
+        lo.y = box_axis(y0, mid);
+        hi.y = box_axis(mid + 1, y1);
+      } else {
+        const int mid = (z0 + z1) >> 1;
+        lo.z = box_axis(z0, mid);
+        hi.z = box_axis(mid + 1, z1);
+      }
+      stack[top++] = hi;
+      stack[top++] = lo;
+      continue;
+    }
+    // one block: its cell rows within the bound, one contiguous run of sorted points per brick a row crosses
+#pragma unroll 1
+    for (int cz = cz0; cz <= cz1; ++cz)
+#pragma unroll 1
+      for (int cy = cy0; cy <= cy1; ++cy) {
+        if (cells_bound(q, cx0, cx1, cy, cy, cz, cz) >= sq_radius) continue;
+        const int rowb = brick_row(g, bs, cy, cz);
+        const uint32_t rowl = cell_row(bs, cy, cz);
+#pragma unroll 1
+        for (int cx = cx0; cx <= cx1;) {
+          const int xe = min(cx1, cx | bs.m);
+          const int rank = __ldg(&g.top[brick_in_row(bs, rowb, cx)]);
+          if (rank >= 0) {
+            const uint32_t s = __ldg(&g.cellStart[cell_in_row(bs, rank, rowl, cx)]);
+            const uint32_t e = __ldg(&g.cellStart[cell_in_row(bs, rank, rowl, xe) + 1u]);
+#pragma unroll 1
+            for (uint32_t k = s; k < e; ++k) {
+              const float4 p = __ldg(&g.pts[k]);
+              const float dx = __fsub_rn(q.tx, p.x), dy = __fsub_rn(q.ty, p.y), dz = __fsub_rn(q.tz, p.z);
+              const float d2 = __fadd_rn(__fmul_rn(dx, dx), __fadd_rn(__fmul_rn(dy, dy), __fmul_rn(dz, dz)));
+              const int i = __float_as_int(p.w);
+              if (d2 < sq_radius && i < q.excl) cluster_unite(parent, i, q.excl);
+            }
+          }
+          cx = xe + 1;
+        }
+      }
+  }
 }
 
 // the segments of one sort chunk (s4g_range): query i's list is [offsets[i], offsets[i + 1]); the chunk takes the lists
@@ -628,6 +743,15 @@ int s4g_launch_radius_count(s4g_ctx* ctx, float sq_radius, int min_neighbors, in
   const int n = ctx->nP;
   k_radius_count<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, 0, ctx->stream>>>(ctx->grid, n, sq_radius,
                                                                                           min_neighbors, d_counts, d_keep);
+  ctx->launches++;
+  S4G_CUDA(cudaGetLastError());
+  return S4G_OK;
+}
+
+int s4g_launch_cluster_link(s4g_ctx* ctx, float sq_radius, int* d_parent) {
+  S4G_CUDA(cudaSetDevice(ctx->device));
+  const int n = ctx->nP;
+  k_cluster_link<<<(unsigned)((n + kThreads - 1) / kThreads), kThreads, 0, ctx->stream>>>(ctx->grid, n, sq_radius, d_parent);
   ctx->launches++;
   S4G_CUDA(cudaGetLastError());
   return S4G_OK;

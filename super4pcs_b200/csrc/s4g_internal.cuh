@@ -374,3 +374,21 @@ int s4g_launch_sorted_queries(s4g_ctx* ctx, float* d_xyz);
 // Enqueue k_radius_count over the resident P (query.cu): d_counts[j] = min(c_j, min_neighbors) (d_counts may be
 // nullptr), d_keep[j] = c_j >= min_neighbors, c_j the number of other P points with d^2 < sq_radius.  min_neighbors >= 1.
 int s4g_launch_radius_count(s4g_ctx* ctx, float sq_radius, int min_neighbors, int32_t* d_counts, uint8_t* d_keep);
+// Enqueue k_cluster_link over the resident P (query.cu): merges, in d_parent [nP] (indexed by original index, parent[x]
+// = x on entry), the two ends of every pair with d^2 < sq_radius; on return each set is a connected component and its
+// root, parent[r] = r, is its smallest index (the other entries point at an ancestor, not yet at the root).
+int s4g_launch_cluster_link(s4g_ctx* ctx, float sq_radius, int* d_parent);
+// The root of x in the union-find forest of the Euclidean clusters (parent[x] <= x, k_cluster_link), halving the path on
+// the way: parent[x] = parent[parent[x]], an ancestor of x.  The accesses go to L2 (ld/st.cg), where the hooks' atomicCAS
+// lands; a value that misses a concurrent write is still an ancestor, so it costs steps only.
+__device__ __forceinline__ int cluster_find(int* parent, int x) {
+  int px = __ldcg(&parent[x]);
+#pragma unroll 1
+  while (px != x) {
+    const int gp = __ldcg(&parent[px]);
+    if (gp != px) __stcg(&parent[x], gp);
+    x = gp;
+    px = __ldcg(&parent[x]);
+  }
+  return x;
+}

@@ -105,6 +105,8 @@ def load_library():
         "s4g_statistical_outliers_dev": ([vp, i32, C.c_double, vp, vp, vp, vp], i32),
         "s4g_radius_outliers": ([vp, f32, i32, vp, vp, vp], i32),
         "s4g_radius_outliers_dev": ([vp, f32, i32, vp, vp, vp], i32),
+        "s4g_euclidean_clusters": ([vp, f32, i32, i32, vp, vp, vp, vp, vp], i32),
+        "s4g_euclidean_clusters_dev": ([vp, f32, i32, i32, vp, vp, vp, vp, vp], i32),
         "s4g_range": ([vp, vp, i32, vp, f32, vp, vp], i32),
         "s4g_get_range": ([vp, vp, vp], i32),
         "s4g_range_count_dev": ([vp, vp, i32, vp, f32, vp], i32),
@@ -149,6 +151,11 @@ def _p(a):
 
 def _c(a, dt=_f):
     return None if a is None else np.ascontiguousarray(a, dtype=dt)
+
+
+def _max_size(max_size):
+    """the max_size argument of s4g_euclidean_clusters: None -> INT_MAX (no limit)"""
+    return 2 ** 31 - 1 if max_size is None else int(max_size)
 
 
 COMM_ID_BYTES = 128
@@ -380,6 +387,30 @@ class Context:
         v = lambda p: C.c_void_p(p) if p else None  # noqa: E731
         self._chk(self._L.s4g_radius_outliers_dev(self.h, float(sq_radius), int(min_neighbors), v(d_keep_ptr),
                                                   v(d_n_kept_ptr), v(d_counts_ptr)))
+
+    def euclidean_clusters(self, sq_radius, min_size=1, max_size=None):
+        """-> (labels [nP] int32, root [nP] int32, offsets [n_clusters + 1] int64, members [offsets[-1]] int32): the
+        connected components of the resident P under d^2 < sq_radius (root[j] = the smallest position in j's component),
+        the clusters among them (min_size <= size <= max_size; None: no upper limit) ordered by size descending, ties by
+        root; labels[j] = the rank of j's cluster or -1; cluster c is members[offsets[c]:offsets[c + 1]], ascending.
+        See s4g.h."""
+        n = self.nP
+        labels, root = np.empty(n, np.int32), np.empty(n, np.int32)
+        offsets, members = np.empty(n + 1, np.int64), np.empty(n, np.int32)
+        nc = C.c_int64(0)
+        self._chk(self._L.s4g_euclidean_clusters(self.h, float(sq_radius), int(min_size), _max_size(max_size), _p(labels),
+                                                 _p(root), C.byref(nc), _p(offsets), _p(members)))
+        nc = nc.value
+        return labels, root, offsets[:nc + 1].copy(), members[:offsets[nc]].copy()
+
+    def euclidean_clusters_dev(self, sq_radius, d_labels_ptr, d_n_clusters_ptr, d_root_ptr=None, d_offsets_ptr=None,
+                               d_members_ptr=None, min_size=1, max_size=None):
+        """device pointers (nP int32 labels, 1 int64 n_clusters, nP int32 root or None, nP + 1 int64 offsets or None, nP
+        int32 members or None), stream-ordered, nothing synchronised"""
+        v = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        self._chk(self._L.s4g_euclidean_clusters_dev(self.h, float(sq_radius), int(min_size), _max_size(max_size),
+                                                     v(d_labels_ptr), v(d_root_ptr), v(d_n_clusters_ptr),
+                                                     v(d_offsets_ptr), v(d_members_ptr)))
 
     def range_query(self, xyz, sq_radius, T=None):
         """-> (offsets [n + 1] int64, indices [total] int32, sq_dist [total] float32): for every query point x, every
