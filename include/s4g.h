@@ -223,6 +223,61 @@ int s4g_euclidean_clusters(s4g_ctx* ctx, float sq_radius, int min_size, int max_
                            int64_t* n_clusters, int64_t* offsets, int32_t* members);
 int s4g_euclidean_clusters_dev(s4g_ctx* ctx, float sq_radius, int min_size, int max_size, int32_t* d_labels,
                                int32_t* d_root, int64_t* d_n_clusters, int64_t* d_offsets, int32_t* d_members);
+/* One plane found by s4g_segment_planes (64 bytes, no padding). */
+typedef struct s4g_plane {
+  float coefficients[4];       /* final (a, b, c, d): a x + b y + c z + d = 0, |(a, b, c)| = 1 in double before rounding */
+  float hypothesis[4];         /* the winning hypothesis' plane, before the refit                                        */
+  int32_t hypothesis_index;    /* its h                                                                                  */
+  int32_t sample[3];           /* its three positions j                                                                  */
+  int64_t hypothesis_inliers;  /* its count                                                                              */
+  int64_t n_inliers;           /* final count = the length of this plane's member list                                  */
+} s4g_plane;
+/* Plane segmentation of the resident sampled P (PCL's SACSegmentation with SACMODEL_PLANE and optimize_coefficients,
+ * made exact): RANSAC with every hypothesis scored, no early termination, so the result is a pure function of (cloud,
+ * threshold, n_hypotheses, seed, refine, max_planes, min_inliers).  j is the position in the array passed to
+ * s4g_set_cloud_p; H = n_hypotheses.
+ *   Rounds r = 0, 1, ..., max_planes - 1.  A_r = the ascending list of the j that no earlier plane claimed (all of P for
+ *   r = 0), m = |A_r|.  m < 3: stop.
+ *   Draws.  seed_r = seed + r (mod 2^64).  Hypothesis h (0 <= h < H) takes draws t = 0, 1, 2; draw t is the k-th
+ *   SplitMix64 output, k = 3h + t + 1 (all mod 2^64):
+ *     z = seed_r + k * 0x9E3779B97F4A7C15;  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9;
+ *     z = (z ^ (z >> 27)) * 0x94D049BB133111EB;  z = z ^ (z >> 31);
+ *   its point is A_r[((z >> 32) * m) >> 32].
+ *   Hypothesis plane, in double from the three float points p0, p1, p2: u = p1 - p0, v = p2 - p0, n = u x v
+ *   (nx = uy vz - uz vy, ny = uz vx - ux vz, nz = ux vy - uy vx), len = sqrt((nx nx + ny ny) + nz nz).  len == 0
+ *   (repeated draws, coincident or collinear points): the hypothesis is invalid and counts 0.  Otherwise n = n / len; if
+ *   n's component of largest magnitude is negative (ties to the lowest axis), n = -n; d = -((nx x0 + ny y0) + nz z0);
+ *   the four values rounded to float.
+ *   Inlier test, fp32, no FMA: r = ((a x + b y) + c z) + d; p is an inlier iff |r| < threshold (strict, as s4g_range
+ *   and PCL's and Open3D's plane models), for the points of A_r only.  hyp_counts[r H + h] = the count of hypothesis h.
+ *   Winner: the valid hypothesis with the largest count, ties to the smallest h.  No valid hypothesis: stop.
+ *   Refit (refine != 0): I = the winner's inliers in ascending j.  In double, c = sum p / |I|, then a second pass C =
+ *   sum (p - c)(p - c)^T / |I|; each sum in this fixed order: the I in ascending j cut into runs of 1024 (the last may be
+ *   shorter), each run summed left to right from 0.0, then the run sums left to right from 0.0.  The eigenvector of C's
+ *   smallest eigenvalue as in s4g_normals (its Jacobi rotations, stable sort and column rule), normalised in double, the
+ *   sign rule above, d = -((nx cx + ny cy) + nz cz), rounded to float.  |I| < 3 or C exactly zero: the hypothesis plane.
+ *   refine == 0: the hypothesis plane.
+ *   Final inliers: the test above with the final coefficients over A_r (PCL's re-selection after its refit).  Plane r is
+ *   accepted iff their number >= min_inliers; otherwise stop (a rejected plane is not reported).  An accepted plane's
+ *   points get labels[j] = r and leave the active set.
+ *   Outputs: labels[j] = the plane that claimed j, -1 for none.  planes[0 .. *n_planes) (capacity max_planes).  Members
+ *   in CSR form: plane r is members[offsets[r] .. offsets[r + 1]), in ascending j (capacities max_planes + 1 and nP;
+ *   only offsets[0 .. n_planes] and members[0 .. offsets[n_planes]) are defined).  hyp_counts: max_planes x H entries,
+ *   the rows of rounds that drew nothing all zero.
+ *   Every count is an integer and every value is made of IEEE basic operations in a stated order, compiled without
+ *   FMA: a CPU restatement compiled without contraction gives the same bits.
+ * threshold not NaN and >= 0 (+inf: every active point), 1 <= n_hypotheses <= 2^20, max_planes >= 1, min_inliers >= 1,
+ * labels, planes and n_planes != NULL; otherwise S4G_ERR_ARG.  offsets, members and hyp_counts may be NULL.  Needs
+ * s4g_set_cloud_p (S4G_ERR_STATE before it); scratch the device cannot hold (37 bytes per P point, 45 in the host form, 36 per
+ * hypothesis, plus CUB's select and radix sort storage) -> S4G_ERR_NOMEM.
+ * _dev: device buffers (d_n_planes one int32), enqueued on the context's stream, nothing synchronised; after a stop the
+ * later rounds are no-ops that read a device flag.                                                                        */
+int s4g_segment_planes(s4g_ctx* ctx, float threshold, int n_hypotheses, uint64_t seed, int refine, int max_planes,
+                       int64_t min_inliers, int32_t* labels, s4g_plane* planes, int* n_planes, int64_t* offsets,
+                       int32_t* members, uint32_t* hyp_counts);
+int s4g_segment_planes_dev(s4g_ctx* ctx, float threshold, int n_hypotheses, uint64_t seed, int refine, int max_planes,
+                           int64_t min_inliers, int32_t* d_labels, s4g_plane* d_planes, int* d_n_planes,
+                           int64_t* d_offsets, int32_t* d_members, uint32_t* d_hyp_counts);
 /* The range query of the reference's kd-tree (KdTree::doQueryDist / doQueryDistIndices / doQueryDistProcessIndices,
  * accelerators/kdtree.h:231-262, body :462-514) on the resident sampled P, for n arbitrary query points xyz (n x 3):
  * the list of query i is every j with d^2 = |y_i - p_j|^2 < sq_radius (strict, the kd-tree's point test kdtree.h:485),

@@ -21,12 +21,12 @@
 // -fmad=false so that no product is contracted into an FMA.  So a CPU restatement of the same operations, compiled
 // without contraction (-ffp-contract=off), gives the same bits.
 #include "s4g_internal.cuh"
+#include "jacobi.cuh"
 #include <cmath>
 
 namespace {
 
 constexpr int kNormalsThreads = 128;
-constexpr int kJacobiSweeps = 50;
 constexpr int kNormalsMinK = 3, kNormalsMaxK = 64;   // k = 64: k_knn's widest instance
 
 // sorted P (float4, w = original index) -> the n x 3 query array of k_knn
@@ -38,43 +38,6 @@ __global__ void k_normals_queries(const float4* __restrict__ pts, int n, float* 
   xyz[3 * t + 1] = p.y;
   xyz[3 * t + 2] = p.z;
 }
-
-// one Givens rotation (x, y) <- (x - s (y + x tau), y + s (x - y tau))
-__device__ __forceinline__ void rotate(double& x, double& y, double s, double tau) {
-  const double g = x, h = y;
-  x = g - s * (h + g * tau);
-  y = h + s * (g - h * tau);
-}
-
-// the Jacobi step of the pair (p, q) of a symmetric 3x3: app, aqq, apq its entries, arp / arq those of the third row r;
-// vp / vq the columns p and q of V.  A negligible apq (100 |apq| lost against both |app| and |aqq|) is set to zero.
-__device__ __forceinline__ void jacobi_pair(double& app, double& aqq, double& apq, double& arp, double& arq, double (&vp)[3],
-                                            double (&vq)[3]) {
-  if (apq == 0.0) return;
-  const double g = 100.0 * fabs(apq);
-  if (fabs(app) + g == fabs(app) && fabs(aqq) + g == fabs(aqq)) {
-    apq = 0.0;
-    return;
-  }
-  const double h = aqq - app;
-  double t;
-  if (fabs(h) + g == fabs(h)) {
-    t = apq / h;
-  } else {
-    const double theta = (0.5 * h) / apq;
-    t = 1.0 / (fabs(theta) + sqrt(theta * theta + 1.0));
-    if (theta < 0.0) t = -t;
-  }
-  const double c = 1.0 / sqrt(t * t + 1.0), s = t * c, tau = s / (1.0 + c), d = t * apq;
-  app = app - d;
-  aqq = aqq + d;
-  apq = 0.0;
-  rotate(arp, arq, s, tau);
-#pragma unroll
-  for (int r = 0; r < 3; ++r) rotate(vp[r], vq[r], s, tau);
-}
-
-__device__ __forceinline__ double pick3(double a, double b, double c, int i) { return i == 0 ? a : i == 1 ? b : c; }
 
 __global__ void __launch_bounds__(kNormalsThreads)
 k_normals(const float4* __restrict__ sorted, const float4* __restrict__ P, const int32_t* __restrict__ rows, int n, int k,
@@ -116,20 +79,8 @@ k_normals(const float4* __restrict__ sorted, const float4* __restrict__ P, const
   a22 = a22 / dm;
   const bool none = m < 3 || (a00 == 0.0 && a01 == 0.0 && a02 == 0.0 && a11 == 0.0 && a12 == 0.0 && a22 == 0.0);
   double v0[3] = {1.0, 0.0, 0.0}, v1[3] = {0.0, 1.0, 0.0}, v2[3] = {0.0, 0.0, 1.0};   // the columns of V
-#pragma unroll 1
-  for (int sweep = 0; sweep < kJacobiSweeps; ++sweep) {
-    if (a01 == 0.0 && a02 == 0.0 && a12 == 0.0) break;
-    jacobi_pair(a00, a11, a01, a02, a12, v0, v1);
-    jacobi_pair(a00, a22, a02, a01, a12, v0, v2);
-    jacobi_pair(a11, a22, a12, a01, a02, v1, v2);
-  }
-  // stable ascending order of the diagonal: o0 <= o1 <= o2, equal values in column order
-  int o0 = 0, o1 = 1, o2 = 2;
-  if (pick3(a00, a11, a22, o1) < pick3(a00, a11, a22, o0)) { const int s = o0; o0 = o1; o1 = s; }
-  if (pick3(a00, a11, a22, o2) < pick3(a00, a11, a22, o1)) {
-    const int s = o1; o1 = o2; o2 = s;
-    if (pick3(a00, a11, a22, o1) < pick3(a00, a11, a22, o0)) { const int s2 = o0; o0 = o1; o1 = s2; }
-  }
+  jacobi_sweeps(a00, a01, a02, a11, a12, a22, v0, v1, v2);
+  S4G_EIGEN_ORDER(a00, a11, a22, o0, o1, o2);
   if (eigenvalues != nullptr) {
     eigenvalues[3 * j] = (float)pick3(a00, a11, a22, o0);
     eigenvalues[3 * j + 1] = (float)pick3(a00, a11, a22, o1);

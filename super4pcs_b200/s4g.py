@@ -42,6 +42,16 @@ class PairFilters(C.Structure):
                 ("max_angle", C.c_float), ("max_color_distance", C.c_float)]
 
 
+class Plane(C.Structure):
+    _fields_ = [("coefficients", C.c_float * 4), ("hypothesis", C.c_float * 4), ("hypothesis_index", C.c_int32),
+                ("sample", C.c_int32 * 3), ("hypothesis_inliers", C.c_int64), ("n_inliers", C.c_int64)]
+
+
+# s4g_plane as a numpy record: Context.segment_planes returns an array of these, one field per struct member
+PLANE_DTYPE = np.dtype([("coefficients", np.float32, 4), ("hypothesis", np.float32, 4), ("hypothesis_index", np.int32),
+                        ("sample", np.int32, 3), ("hypothesis_inliers", np.int64), ("n_inliers", np.int64)])
+assert PLANE_DTYPE.itemsize == C.sizeof(Plane) == 64
+
 _lib = None
 
 
@@ -107,6 +117,8 @@ def load_library():
         "s4g_radius_outliers_dev": ([vp, f32, i32, vp, vp, vp], i32),
         "s4g_euclidean_clusters": ([vp, f32, i32, i32, vp, vp, vp, vp, vp], i32),
         "s4g_euclidean_clusters_dev": ([vp, f32, i32, i32, vp, vp, vp, vp, vp], i32),
+        "s4g_segment_planes": ([vp, f32, i32, C.c_uint64, i32, i32, i64, vp, C.POINTER(Plane), vp, vp, vp, vp], i32),
+        "s4g_segment_planes_dev": ([vp, f32, i32, C.c_uint64, i32, i32, i64, vp, vp, vp, vp, vp, vp], i32),
         "s4g_range": ([vp, vp, i32, vp, f32, vp, vp], i32),
         "s4g_get_range": ([vp, vp, vp], i32),
         "s4g_range_count_dev": ([vp, vp, i32, vp, f32, vp], i32),
@@ -411,6 +423,39 @@ class Context:
         self._chk(self._L.s4g_euclidean_clusters_dev(self.h, float(sq_radius), int(min_size), _max_size(max_size),
                                                      v(d_labels_ptr), v(d_root_ptr), v(d_n_clusters_ptr),
                                                      v(d_offsets_ptr), v(d_members_ptr)))
+
+    def segment_planes(self, threshold, n_hypotheses=1000, max_planes=1, min_inliers=1, seed=0, refine=True,
+                       hyp_counts=False):
+        """-> (labels [nP] int32, planes [n_planes] PLANE_DTYPE, offsets [n_planes + 1] int64, members [offsets[-1]]
+        int32), and counts [max_planes, n_hypotheses] uint32 when hyp_counts: RANSAC planes of the resident P, every
+        hypothesis counted (inlier iff |a x + b y + c z + d| < threshold in fp32), the winner refitted by least squares
+        (refine), up to max_planes planes of at least min_inliers points each, one after the other on the points no
+        earlier plane claimed.  labels[j] = the plane of position j or -1; plane r is members[offsets[r]:offsets[r + 1]],
+        ascending.  A pure function of its arguments; see s4g.h (s4g_segment_planes)."""
+        n, H, R = self.nP, int(n_hypotheses), int(max_planes)
+        labels, members = np.empty(n, np.int32), np.empty(n, np.int32)
+        planes, offsets = np.zeros(max(R, 0), PLANE_DTYPE), np.zeros(max(R, 0) + 1, np.int64)
+        counts = np.empty((max(R, 0), max(H, 0)), np.uint32) if hyp_counts else None
+        np_ = C.c_int(0)
+        self._chk(self._L.s4g_segment_planes(self.h, float(threshold), H, C.c_uint64(int(seed) % 2 ** 64),
+                                             1 if refine else 0, R, int(min_inliers), _p(labels),
+                                             planes.ctypes.data_as(C.POINTER(Plane)), C.byref(np_), _p(offsets),
+                                             _p(members), _p(counts)))
+        k = np_.value
+        out = (labels, planes[:k].copy(), offsets[:k + 1].copy(), members[:offsets[k]].copy())
+        return out + (counts,) if hyp_counts else out
+
+    def segment_planes_dev(self, threshold, d_labels_ptr, d_planes_ptr, d_n_planes_ptr, d_offsets_ptr=None,
+                           d_members_ptr=None, d_hyp_counts_ptr=None, n_hypotheses=1000, max_planes=1, min_inliers=1,
+                           seed=0, refine=True):
+        """device pointers (nP int32 labels, max_planes 64-byte s4g_plane records, 1 int32 n_planes, max_planes + 1
+        int64 offsets or None, nP int32 members or None, max_planes x n_hypotheses uint32 counts or None),
+        stream-ordered, nothing synchronised"""
+        v = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        self._chk(self._L.s4g_segment_planes_dev(self.h, float(threshold), int(n_hypotheses),
+                                                 C.c_uint64(int(seed) % 2 ** 64), 1 if refine else 0, int(max_planes),
+                                                 int(min_inliers), v(d_labels_ptr), v(d_planes_ptr), v(d_n_planes_ptr),
+                                                 v(d_offsets_ptr), v(d_members_ptr), v(d_hyp_counts_ptr)))
 
     def range_query(self, xyz, sq_radius, T=None):
         """-> (offsets [n + 1] int64, indices [total] int32, sq_dist [total] float32): for every query point x, every
