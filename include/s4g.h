@@ -394,7 +394,9 @@ int s4g_get_quads(s4g_ctx* ctx, int32_t* out_quads /* 4*n */);
  * dimension / a key prefix of every kernel, the lists of all bases share buffers, sizes stay on the device, and the
  * host reads back once per stage (3 per batch instead of ~7 per base).  Per base the result equals the per-base
  * chain's (same pair sets, same quads in the same order, same winner).  Limits: n_bases <= 64, |sampled_Q| < 2^26,
- * distance_threshold2 / _ratio >= 2^-14; beyond them S4G_ERR_ARG (callers fall back to the per-base chain).
+ * fewer than 2^26 pairs in every extraction (the quad keys hold a pair's index in 26 bits), quad grid depth <= 14
+ * (distance_threshold2 / _ratio above about 2^-15); beyond them S4G_ERR_ARG.  More than 2^32 - 1 pairs or 2^31 - 1
+ * quads in one batch: S4G_ERR_NOMEM.  Callers fall back to the per-base chain on either code.
  * The resident pair slots / quads of the context are left untouched.                                              */
 typedef struct s4g_base_desc {
   float pair_distance[2];       /* |b0-b1|, |b2-b3|                                        */

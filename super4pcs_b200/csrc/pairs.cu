@@ -653,6 +653,9 @@ int s4g_batch_pairs(s4g_ctx* ctx, const s4g_base_desc* bases, int B, float eps, 
     S4G_CUDA(cudaGetLastError());
     S4G_CUDA(cudaMemcpyAsync(&h, d_total, 8 + 4 * (size_t)nSeg, cudaMemcpyDeviceToHost, st));
     S4G_CUDA(cudaStreamSynchronize(st));                                         // read-back 1 of 3
+    // the batched quad keys hold a pair's index inside its extraction in 26 bits (base << 52 | id << 26 | i)
+    for (int s = 0; s < nSeg; ++s)
+      if (h.seg[s] >= (1u << kBatchIdBits)) { ctx->err = "s4g_try_bases: an extraction has 2^26 or more pairs"; return S4G_ERR_ARG; }
     if (h.total <= cap) break;
     if (h.total >= (1ull << 32)) { ctx->err = "s4g_try_bases: more than 2^32-1 ordered pairs in one batch"; return S4G_ERR_NOMEM; }
     S4G_TRY(s4g_reserve(ctx, ctx->bPairKeys[0], (size_t)h.total * sizeof(unsigned long long)));

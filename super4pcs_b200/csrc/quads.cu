@@ -524,7 +524,8 @@ int s4g_batch_quads(s4g_ctx* ctx, const s4g_base_desc* bases, float thr2, BatchH
   const unsigned long long* pkeys = ctx->bPairKeys[1].as<unsigned long long>();
   S4G_TRY(s4g_reserve(ctx, ctx->bArgs, std::max<size_t>(args.size() * sizeof(QuadArgs), 64 * 1024)));
   S4G_TRY(s4g_reserve(ctx, ctx->bMisc, 4096));
-  uint32_t* d_segOff = ctx->bMisc.as<uint32_t>();                 // [0 .. 2B]: segment offsets, [256 ..]: quad offsets, [512]: error flag
+  uint32_t* d_segOff = ctx->bMisc.as<uint32_t>();                 // [0 .. 2B]: segment offsets, [256 ..]: quad offsets, [512]: error flag,
+                                                                   // [520, 522): 64-bit quad total
   uint32_t* d_quadOff = d_segOff + 256;
   uint32_t* d_err = d_segOff + 512;
   S4G_CUDA(cudaMemcpyAsync(ctx->bArgs.p, args.data(), args.size() * sizeof(QuadArgs), cudaMemcpyHostToDevice, st));
@@ -558,20 +559,27 @@ int s4g_batch_quads(s4g_ctx* ctx, const s4g_base_desc* bases, float thr2, BatchH
   S4G_TRY(s4g_reserve(ctx, ctx->dCub, scan_bytes));
   cub::DeviceScan::ExclusiveSum(ctx->dCub.p, scan_bytes, counts, offsets, (long long)(n + 1), st);
   k_bquad_offsets<<<1, 128, 0, st>>>(offsets, d_segOff, B, n, d_quadOff);
-  ctx->launches += 6;
+  // the 32-bit offsets wrap once the batch has 2^32 quads: their total is summed again in 64 bits
+  unsigned long long* d_total = reinterpret_cast<unsigned long long*>(d_segOff + 520);
+  size_t sum_bytes = 0;
+  cub::DeviceReduce::Sum(nullptr, sum_bytes, counts, d_total, n, st);
+  S4G_TRY(s4g_reserve(ctx, ctx->dCub, sum_bytes));
+  cub::DeviceReduce::Sum(ctx->dCub.p, sum_bytes, counts, d_total, n, st);
+  ctx->launches += 7;
   S4G_CUDA(cudaGetLastError());
   uint32_t herr = 0;
+  unsigned long long total = 0;
   S4G_CUDA(cudaMemcpyAsync(bh.quadOff, d_quadOff, (size_t)(B + 1) * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   S4G_CUDA(cudaMemcpyAsync(&herr, d_err, 4, cudaMemcpyDeviceToHost, st));
+  S4G_CUDA(cudaMemcpyAsync(&total, d_total, sizeof total, cudaMemcpyDeviceToHost, st));
   S4G_CUDA(cudaStreamSynchronize(st));                              // read-back 2 of 3
   if (herr) { ctx->err = "s4g_try_bases: internal error (quad cell key exceeds 52 bits)"; return S4G_ERR_CUDA; }
-  const unsigned long long total = bh.quadOff[B];
+  if (total >= (1ull << 31)) { ctx->err = "s4g_try_bases: more than 2^31-1 quads in one batch"; return S4G_ERR_NOMEM; }
   bh.nQuads = total;
   if (total == 0) {
     S4G_EV_STOP(ctx, S4G_EV_QUADS);
     return S4G_OK;
   }
-  if (total >= (1ull << 31)) { ctx->err = "s4g_try_bases: more than 2^31-1 quads in one batch"; return S4G_ERR_NOMEM; }
   for (int k = 0; k < 2; ++k) S4G_TRY(s4g_reserve(ctx, ctx->bQuadKeys[k], (size_t)total * sizeof(unsigned long long)));
   S4G_TRY(s4g_reserve(ctx, ctx->bQuads, (size_t)total * sizeof(int4)));
   unsigned long long* qk_in = ctx->bQuadKeys[0].as<unsigned long long>();

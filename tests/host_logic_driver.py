@@ -150,6 +150,15 @@ def run(which, libpath):
             rows.append([bool(np.float32(score) == g["c%d_score" % k]),
                          bool(np.array_equal(T.view(np.uint32), g["c%d_T" % k].view(np.uint32)))])
         out = dict(rows=rows)
+    elif which == "bigpairs":
+        # a base whose one diagonal's pair band covers every pair of a line of 8200 points (67,231,800 >= 2^26 ordered
+        # pairs) and whose other diagonal's band holds none: the batched pass must refuse it and the per-base chain take it
+        Q = np.zeros((8200, 3), np.float32)
+        Q[:, 0] = np.linspace(-0.49, 0.49, 8200, dtype=np.float32)
+        P = np.array([[-0.25, 0, 0], [0.25, 0, 0], [0, 0.75, 0], [0, -0.75, 0]], np.float32)   # diagonals 0.5 and 1.5
+        opt = oref.make_options(delta=0.25, overlap=1.0, sample_size=10 ** 6, max_time_seconds=10000, random_seed=5)
+        score, T, Qt = oref.compute_transformation(P, Q, opt, libpath=libpath)
+        out = dict(score=float(np.float32(score)), T=[int(x) for x in T.view(np.uint32)], Q=_h(Qt))
     elif which == "pairtest":
         # the reference's own ExtractPairs test (tests/pair_extraction.cc:239-314) through MatchSuper4PCS::ExtractPairs
         from tests.test_oracle_golden import _bruteforce_pairs, _sphere_cloud
