@@ -419,6 +419,40 @@ int s4g_try_bases(s4g_ctx* ctx, const s4g_base_desc* bases, int n_bases, float p
  * receives the kept input indices in ascending order (= the reference's output order).      */
 int s4g_voxel_sample(s4g_ctx* ctx, const float* xyz, int64_t n, float voxel, int32_t* out_indices,
                      int64_t* n_out);
+/* Voxel-grid downsampling to centroids (PCL's VoxelGrid with setMinimumPointsNumberPerVoxel, Open3D's voxel_down_sample
+ * with its trace, made exact) of n arbitrary points xyz (n x 3; no resident cloud needed: it shrinks a cloud before
+ * s4g_set_cloud_p).  i is the input index.
+ *   Voxel of a point: (floor(x s), floor(y s), floor(z s)) with s = 1.0f / leaf and each product one fp32 rounding, the
+ *   arithmetic of s4g_voxel_sample (and PCL's).  The key is 3 x 21 bits, relative to the voxel of the bounding-box
+ *   minimum, as in s4g_voxel_sample.  A coordinate that is not finite, a scaled coordinate whose floor is outside the
+ *   int32 range, or a span of 2^21 or more voxels along an axis -> S4G_ERR_ARG.
+ *   Members of a voxel: its points in ascending i; m their number.  A voxel with m < min_points is dropped.
+ *   Sums, in double, each in this fixed order: the members cut into runs of 1024 (the last may be shorter), each run
+ *   summed left to right from 0.0, then the run sums left to right from 0.0.  Only + - * /, sqrt and comparisons, no
+ *   FMA: a CPU restatement compiled without contraction gives the same bits.
+ *     centroid = (sum p) / m, rounded to float;  rgb = (sum rgb) / m, rounded to float;
+ *     normal: S = sum n, len = sqrt((Sx Sx + Sy Sy) + Sz Sz); len == 0: (0, 0, 0), which the pair filter reads as "no
+ *     normal"; otherwise S / len, rounded to float.  Zero normals add nothing; opposite normals cancel, so averaging
+ *     assumes consistently oriented normals: the recommended chain downsamples first and estimates normals afterwards.
+ *   Output order: the surviving voxels in ascending order of their first (smallest) member i, i.e. input order.
+ *     xyz_out / normals_out / rgb_out [v] as above; counts[v] = m; first[v] = the smallest member i (with min_points = 1
+ *     exactly the output of s4g_voxel_sample); voxel_of[i] = the output index of i's voxel, -1 when it was dropped
+ *     (Open3D's trace: it averages any other attribute).  *n_out = the number of surviving voxels.
+ *   normals / normals_out and rgb / rgb_out are pairs, both NULL or both given; counts, first and voxel_of may be NULL.
+ *   Output capacity n (voxel_of: n entries).  leaf finite and > 0, min_points >= 1, 0 <= n < 2^31, xyz, xyz_out and
+ *   n_out != NULL; otherwise S4G_ERR_ARG.  n == 0: *n_out = 0.
+ *   Device scratch: 36 bytes per point plus 12 per attribute array given (48 for xyz alone, 72 with normals and rgb),
+ *   plus CUB's radix sort and scan storage; the host form also holds its inputs and outputs on the device (12 bytes
+ *   per point per attribute array each way, 4 per index array).  Scratch the device cannot hold -> S4G_ERR_NOMEM.
+ * _dev: device buffers (d_n_out one int64), enqueued on the context's stream, nothing synchronised.  So an invalid
+ * coordinate or too wide a span cannot be returned as a code: the call then writes *d_n_out = -1 and the outputs are
+ * undefined.                                                                                                            */
+int s4g_voxel_grid(s4g_ctx* ctx, const float* xyz, const float* normals, const float* rgb, int64_t n, float leaf,
+                   int min_points, float* xyz_out, float* normals_out, float* rgb_out, int32_t* counts, int32_t* first,
+                   int32_t* voxel_of, int64_t* n_out);
+int s4g_voxel_grid_dev(s4g_ctx* ctx, const float* d_xyz, const float* d_normals, const float* d_rgb, int64_t n, float leaf,
+                       int min_points, float* d_xyz_out, float* d_normals_out, float* d_rgb_out, int32_t* d_counts,
+                       int32_t* d_first, int32_t* d_voxel_of, int64_t* d_n_out);
 
 /* ---- row e (SURVEY.md 8(e)): the reduction of a sharded candidate set inside the library -----------------------------
  * The reference runs the candidates of a base through one loop (OpenMP-optional, match4pcsBase.hpp:390-393, strict '>' in

@@ -145,6 +145,8 @@ def load_library():
         "s4g_get_quads": ([vp, vp], i32),
         "s4g_get_timings": ([vp, vp], i32),
         "s4g_voxel_sample": ([vp, vp, i64, f32, vp, C.POINTER(i64)], i32),
+        "s4g_voxel_grid": ([vp, vp, vp, vp, i64, f32, i32, vp, vp, vp, vp, vp, vp, C.POINTER(i64)], i32),
+        "s4g_voxel_grid_dev": ([vp, vp, vp, vp, i64, f32, i32, vp, vp, vp, vp, vp, vp, vp], i32),
     }
     for name, (args, res) in sig.items():
         try:
@@ -628,6 +630,41 @@ class Context:
         n = C.c_int64(0)
         self._chk(self._L.s4g_voxel_sample(self.h, _p(X), len(X), float(voxel), _p(out), C.byref(n)))
         return out[:n.value].copy()
+
+    def voxel_grid(self, xyz, leaf, normals=None, rgb=None, min_points=1):
+        """-> (centroids [m, 3] float32, normals [m, 3] float32 or None, rgb [m, 3] float32 or None, counts [m] int32,
+        first [m] int32, voxel_of [n] int32): the voxel grid of edge `leaf` downsampled to one centroid per voxel with at
+        least min_points points, the normal and colour averaged over the same points, in the order of each voxel's first
+        point; voxel_of[i] = the output row of point i's voxel or -1.  Fixed-order double sums; see s4g.h
+        (s4g_voxel_grid)."""
+        X = _c(xyz).reshape(-1, 3)
+        N = None if normals is None else _c(normals).reshape(-1, 3)
+        R = None if rgb is None else _c(rgb).reshape(-1, 3)
+        n = len(X)
+        for a in (N, R):
+            if a is not None and len(a) != n:
+                raise ValueError("normals and rgb need one row per point")
+        out = np.empty((n, 3), np.float32)
+        nout = None if N is None else np.empty((n, 3), np.float32)
+        rout = None if R is None else np.empty((n, 3), np.float32)
+        counts, first, voxel_of = np.empty(n, np.int32), np.empty(n, np.int32), np.empty(n, np.int32)
+        m = C.c_int64(0)
+        self._chk(self._L.s4g_voxel_grid(self.h, _p(X), _p(N), _p(R), n, float(leaf), int(min_points), _p(out),
+                                         _p(nout), _p(rout), _p(counts), _p(first), _p(voxel_of), C.byref(m)))
+        k = m.value
+        cut = lambda a: None if a is None else a[:k].copy()  # noqa: E731
+        return out[:k].copy(), cut(nout), cut(rout), counts[:k].copy(), first[:k].copy(), voxel_of
+
+    def voxel_grid_dev(self, d_xyz_ptr, n, leaf, d_xyz_out_ptr, d_n_out_ptr, d_normals_ptr=None, d_rgb_ptr=None,
+                       d_normals_out_ptr=None, d_rgb_out_ptr=None, d_counts_ptr=None, d_first_ptr=None,
+                       d_voxel_of_ptr=None, min_points=1):
+        """device pointers (n x 3 float32 inputs; outputs of capacity n; 1 int64 n_out, -1 for an invalid coordinate or
+        span), stream-ordered, nothing synchronised"""
+        v = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        self._chk(self._L.s4g_voxel_grid_dev(self.h, v(d_xyz_ptr), v(d_normals_ptr), v(d_rgb_ptr), int(n), float(leaf),
+                                             int(min_points), v(d_xyz_out_ptr), v(d_normals_out_ptr),
+                                             v(d_rgb_out_ptr), v(d_counts_ptr), v(d_first_ptr), v(d_voxel_of_ptr),
+                                             v(d_n_out_ptr)))
 
     # ---- a4 / a5
     def find_quads(self, inv1, inv2, thr2, base_xyz, fetch=True):
