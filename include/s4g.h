@@ -167,6 +167,39 @@ int s4g_knn_probe_stats(s4g_ctx* ctx, const float* xyz, int n, const float* T_co
  * floats (or NULL), read before the call returns.                                                                      */
 int s4g_normals(s4g_ctx* ctx, int k, float sq_radius, const float* viewpoint, float* normals, float* eigenvalues);
 int s4g_normals_dev(s4g_ctx* ctx, int k, float sq_radius, const float* viewpoint, float* d_normals, float* d_eigenvalues);
+/* Consistent orientation of the normals of the resident sampled P (Hoppe et al. 1992; Open3D's
+ * orient_normals_consistent_tangent_plane), made exact: signs propagated along the minimum spanning forest of the
+ * symmetrised k-nearest graph.  j is the position in the array passed to s4g_set_cloud_p; normals holds nP x 3 floats in
+ * that order (what s4g_normals writes); any non-zero vector is a normal, its length does not matter.
+ *   Vertices: the points whose normal is not (0, 0, 0).  The others keep it, get root[j] = -1 and belong to no component.
+ *   Edges: row j is exactly the s4g_knn row of the query p_j with exclude = j, no T, the caller's k and sq_radius; the
+ *   undirected edge {i, j} exists iff j is in row i or i is in row j, and both ends are vertices (padding skipped).
+ *   Edge values, fp32, no FMA, from the input normals: dot = (xi xj + yi yj) + zi zj (the same float from either end);
+ *   flip f(i, j) = dot < 0 (strict: 0 and -0 are no flip).
+ *   Order: |dot| descending, then lo = min(i, j) ascending, then hi = max(i, j) ascending (Hoppe's weight 1 - |dot|
+ *   without the rounding of 1 - x).  It is total, so the minimum spanning forest is unique.  A NaN dot (products that
+ *   overflow to opposite infinities) ranks above +inf and is no flip.
+ *   Components: those of the graph; root[j] = the smallest j in j's component (the rule of s4g_euclidean_clusters).
+ *   Anchor of a component: without a viewpoint, its root, which keeps the sign of its input normal; with a viewpoint v
+ *   (3 finite floats), the member with the smallest d^2 = dx^2 + (dy^2 + dz^2), d = p - v in fp32 without FMA, ties to
+ *   the smallest j, whose normal is negated when (v - p_a) . n_a < 0 in double (s4g_normals' viewpoint rule).
+ *   Output: normals_out[j] = the input normal, negated iff (the anchor's negation) xor (the xor of f over the edges of the
+ *   forest path from the anchor to j).  Every output float is + or - its input float, bit for bit.
+ *   out2 = {n_components, n_tree_edges}, n_tree_edges = (number of vertices) - n_components.  tree_edges: the forest as
+ *   (lo, hi) int32 pairs in ascending (lo, hi), capacity 2 (nP - 1) int32.  root and tree_edges may be NULL.
+ *   Every output is integer work on the forest, which the edge set and the order fix, plus one double comparison per
+ *   component: the same bits on every run.
+ * 1 <= k <= 64, sq_radius >= 0 and not NaN (+inf = unbounded), normals, normals_out and out2 != NULL, viewpoint NULL or
+ * finite; otherwise S4G_ERR_ARG.  A normal component that is not finite -> S4G_ERR_ARG.  normals_out may equal normals
+ * (in place).  Needs s4g_set_cloud_p (S4G_ERR_STATE before it); scratch the device cannot hold (nP x (k + 13) 4-byte
+ * words plus CUB's radix sort storage, and 24 more bytes per point in the host form) -> S4G_ERR_NOMEM.
+ * _dev: device buffers (d_out2 two int64), enqueued on the context's stream, nothing synchronised; viewpoint is 3 host
+ * floats (or NULL), read before the call returns.  A non-finite normal component cannot be returned as a code: the call
+ * then writes d_out2[0] = -1 and the other outputs are undefined.                                                      */
+int s4g_orient_normals(s4g_ctx* ctx, const float* normals, int k, float sq_radius, const float* viewpoint,
+                       float* normals_out, int32_t* root, int64_t* out2, int32_t* tree_edges);
+int s4g_orient_normals_dev(s4g_ctx* ctx, const float* d_normals, int k, float sq_radius, const float* viewpoint,
+                           float* d_normals_out, int32_t* d_root, int64_t* d_out2, int32_t* d_tree_edges);
 /* Outlier removal on the resident sampled P.  j is the position in the array passed to s4g_set_cloud_p.  Both filters
  * write the kept j in ascending order to keep[0 .. *n_kept) (capacity nP; the output form of s4g_voxel_sample).
  *

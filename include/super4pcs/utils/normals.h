@@ -36,6 +36,27 @@ int EstimateNormals(std::vector<Point3D>& cloud, int k,
                     Point3D::Scalar max_distance = std::numeric_limits<Point3D::Scalar>::infinity(),
                     const Point3D::VectorType* viewpoint = nullptr);
 
+/// Orients the normals of `cloud` consistently, on the GPU by s4g_orient_normals (Hoppe et al. 1992; Open3D's
+/// orient_normals_consistent_tangent_plane), and returns the number of components.  The k-nearest graph of the points
+/// (each point's k nearest other points within max_distance, squared in fp32; +inf: unbounded), made symmetric and
+/// restricted to the points with a non-zero normal, is weighted by |n_i . n_j|; signs propagate along its minimum
+/// spanning forest (largest |n_i . n_j| first, ties by index), flipping where n_i . n_j < 0.  Each component keeps the
+/// sign of one anchor: its smallest index, or with a viewpoint the point nearest to it, turned to face it (the rule of
+/// EstimateNormals).  So with a viewpoint outside a closed surface sampled densely enough, every normal points outward,
+/// which the per-point viewpoint rule cannot give for points that face away from it.  Points with a zero normal keep it.
+///
+///   Utils::EstimateNormals(P, 16);                 // on the dense cloud, where the PCA has the most support
+///   Utils::OrientNormals(P, 16, inf, &viewpoint);  // consistent signs
+///   Utils::VoxelGridFilter(P, 0.005f);             // the averaged normals no longer cancel
+///
+/// A flipped normal is stored as set_normal(-normal()), which renormalises in float: its last bit may move.  Normals
+/// that keep their sign are not touched.  The short-lived context and its grid's delta are EstimateNormals'.
+/// 1 <= k <= 64.  Throws std::runtime_error when k or max_distance is out of range, a normal is not finite or the device
+/// fails; the cloud is then unchanged.
+int OrientNormals(std::vector<Point3D>& cloud, int k,
+                  Point3D::Scalar max_distance = std::numeric_limits<Point3D::Scalar>::infinity(),
+                  const Point3D::VectorType* viewpoint = nullptr);
+
 }  // namespace Utils
 }  // namespace GlobalRegistration
 

@@ -111,6 +111,8 @@ def load_library():
         "s4g_knn_probe_stats": ([vp, vp, i32, vp, i32, f32, vp, vp, vp, vp], i32),
         "s4g_normals": ([vp, i32, f32, vp, vp, vp], i32),
         "s4g_normals_dev": ([vp, i32, f32, vp, vp, vp], i32),
+        "s4g_orient_normals": ([vp, vp, i32, f32, vp, vp, vp, vp, vp], i32),
+        "s4g_orient_normals_dev": ([vp, vp, i32, f32, vp, vp, vp, vp, vp], i32),
         "s4g_statistical_outliers": ([vp, i32, C.c_double, vp, vp, vp, vp], i32),
         "s4g_statistical_outliers_dev": ([vp, i32, C.c_double, vp, vp, vp, vp], i32),
         "s4g_radius_outliers": ([vp, f32, i32, vp, vp, vp], i32),
@@ -366,6 +368,34 @@ class Context:
         vp = None if viewpoint is None else _c(viewpoint).reshape(3)
         self._chk(self._L.s4g_normals_dev(self.h, int(k), float(sq_radius), _p(vp), v(d_normals_ptr),
                                           v(d_eigenvalues_ptr)))
+
+    def orient_normals(self, normals, k, sq_radius=np.inf, viewpoint=None):
+        """-> (oriented [nP, 3] float32, root [nP] int32, n_components, tree_edges [n_tree, 2] int32): the normals of the
+        resident P (one row per point, in the order of set_cloud_p; (0, 0, 0) = no normal) with their signs made
+        consistent along the minimum spanning forest of the k-nearest graph weighted by |n_i . n_j|; root[j] = the
+        smallest position in j's component (-1: no normal); each component's anchor (its root, or with a viewpoint the
+        member nearest to it, turned to face it) keeps its sign.  The forest is returned in ascending (lo, hi).
+        1 <= k <= 64; see s4g.h (s4g_orient_normals)."""
+        n = self.nP
+        N = _c(normals).reshape(-1, 3)
+        if len(N) != n:
+            raise ValueError("orient_normals needs one normal per resident P point")
+        vp = None if viewpoint is None else _c(viewpoint).reshape(3)
+        out, root = np.empty((n, 3), _f), np.empty(n, np.int32)
+        tree, out2 = np.empty((max(n - 1, 0), 2), np.int32), np.zeros(2, np.int64)
+        self._chk(self._L.s4g_orient_normals(self.h, _p(N), int(k), float(sq_radius), _p(vp), _p(out), _p(root),
+                                             _p(out2), _p(tree)))
+        return out, root, int(out2[0]), tree[:int(out2[1])].copy()
+
+    def orient_normals_dev(self, d_normals_ptr, k, d_normals_out_ptr, d_out2_ptr, d_root_ptr=None, d_tree_edges_ptr=None,
+                           sq_radius=np.inf, viewpoint=None):
+        """device pointers (nP x 3 float32 normals in and out, which may be the same buffer; 2 int64 out2 = {n_components
+        or -1 for a non-finite normal, n_tree_edges}; nP int32 root and 2 (nP - 1) int32 tree_edges or None),
+        stream-ordered, nothing synchronised; viewpoint: 3 floats or None, as in orient_normals"""
+        v = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        vp = None if viewpoint is None else _c(viewpoint).reshape(3)
+        self._chk(self._L.s4g_orient_normals_dev(self.h, v(d_normals_ptr), int(k), float(sq_radius), _p(vp),
+                                                 v(d_normals_out_ptr), v(d_root_ptr), v(d_out2_ptr), v(d_tree_edges_ptr)))
 
     def statistical_outliers(self, k, std_ratio):
         """-> (keep [n_kept] int32, mean_dist [nP] float64, mu, sigma): the resident P points (positions in the array of
