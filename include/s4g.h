@@ -200,6 +200,56 @@ int s4g_orient_normals(s4g_ctx* ctx, const float* normals, int k, float sq_radiu
                        float* normals_out, int32_t* root, int64_t* out2, int32_t* tree_edges);
 int s4g_orient_normals_dev(s4g_ctx* ctx, const float* d_normals, int k, float sq_radius, const float* viewpoint,
                            float* d_normals_out, int32_t* d_root, int64_t* d_out2, int32_t* d_tree_edges);
+/* FPFH descriptors of the resident sampled P (Rusu et al. 2009; PCL's FPFHEstimation, Open3D's compute_fpfh_feature),
+ * made exact.  j is the position in the array passed to s4g_set_cloud_p; normals holds nP x 3 floats in that order (what
+ * s4g_normals writes); fpfh receives nP x 33 floats in the same order: bins 0-10 f1, 11-21 f2, 22-32 f3.  The descriptors
+ * depend on the signs of the normals (negating them all mirrors the f1 and f3 blocks), so orient them consistently first
+ * (s4g_orient_normals).
+ *   Row of j: exactly the s4g_knn row of the query p_j with exclude = j, no T, the caller's k and sq_radius, in ascending
+ *   (d^2, index), padding skipped, d^2 the float s4g_knn returns (Open3D's hybrid search with max_nn = k + 1).
+ *   Normals: (0, 0, 0) or a non-finite component is no normal; any other is divided by sqrt(n . n) in double.  A point
+ *   without a normal gets an all-zero descriptor; row entries without a normal are left out, and m_j is the number of
+ *   entries that remain.
+ *   Arithmetic: double, from the float inputs, + - * /, sqrt, floor and comparisons only, no FMA; every dot product is
+ *   (a0 b0 + a1 b1) + a2 b2 and every cross product the textbook component formula.
+ *   Pair feature of (p1, n1) = (p_j, n_j), (p2, n2) = (p_e, n_e) (Open3D's ComputePairFeatures with its two rounded
+ *   transcendental decisions made exact): dp = p2 - p1, d = sqrt(dp . dp), degenerate if d = 0; a1 = n1 . dp / d,
+ *   a2 = n2 . dp / d; swap iff |a1| < |a2| (Open3D's acos(|a1|) > acos(|a2|)): then (u, n') = (n2, n1), dp = -dp and
+ *   f3 = -a2, else (u, n') = (n1, n2) and f3 = a1; v = dp x u, degenerate if |v| = 0, else v = v / |v|; w = u x v;
+ *   f2 = v . n'; the f1 direction is (x, y) = (u . n', w . n').  A degenerate pair lands in bins (5, 16, 27).
+ *   Bins: f2, f3: floor(11 * (f + 1.0) * 0.5) left to right, clamped to [0, 10].  f1: floor(11 (atan2(y, x) + pi) / 2pi)
+ *   replaced by exact half-plane tests against beta_i = -pi + 2 pi i / 11, c_i = cos beta_i and s_i = sin beta_i correctly
+ *   rounded to double, c_{11-i} = c_i and s_{11-i} = -s_i:
+ *     i = 1: c -0x1.aeb8c8764f0bap-1, s -0x1.14cedf8bb580bp-1    i = 4: c 0x1.4f49e7f775887p-1, s -0x1.82f19bb3a28a1p-1
+ *     i = 2: c -0x1.a9628d9c712b6p-2, s -0x1.d1bb48eee2c13p-1    i = 5: c 0x1.eb42a9bcd5057p-1, s -0x1.207e7fd768dbfp-2
+ *     i = 3: c  0x1.2375f640f44dbp-3, s -0x1.fac9e043842efp-1
+ *   y = 0 (either sign): bin 10 if x < 0, else 5; y > 0: 5 + #{i in 6..10 : c_i y - s_i x >= 0};
+ *   y < 0: #{i in 1..5 : c_i y - s_i x >= 0}.
+ *   SPFH of j: cnt_j[b] the pairs of j's row in bin b; spfh_j[b] = (100.0 cnt_j[b]) / m_j (all zero when m_j = 0).
+ *   FPFH of j: acc[b] = the sum, over the entries e of j's row with d^2_e > 0, in row order from 0.0, of
+ *   spfh_e[b] / d^2_e (the inverse squared distance, as PCL's and Open3D's code weigh); S_h = acc[11h] + ... + acc[11h+10]
+ *   left to right; fpfh[j][b] = (float)(acc[b] * (100.0 / S_h) + spfh_j[b]), or (float)spfh_j[b] when S_h = 0.  Open3D
+ *   sums S_h interleaved with acc; the per-bin form lets bins be reduced independently and differs only in rounding.
+ *   Every output is fixed by these operations: the same bits on every run and on a CPU restatement without contraction.
+ * 1 <= k <= 64, sq_radius >= 0 and not NaN (+inf = unbounded), normals and fpfh != NULL; otherwise S4G_ERR_ARG.  Needs
+ * s4g_set_cloud_p (S4G_ERR_STATE before it); scratch the device cannot hold (nP x (8k + 48) bytes, and nP x 144 more in
+ * the host form) -> S4G_ERR_NOMEM.
+ * _dev: device buffers, enqueued on the context's stream, nothing synchronised.                                       */
+int s4g_fpfh(s4g_ctx* ctx, const float* normals, int k, float sq_radius, float* fpfh);
+int s4g_fpfh_dev(s4g_ctx* ctx, const float* d_normals, int k, float sq_radius, float* d_fpfh);
+/* Nearest descriptor by brute force (Open3D's correspondence search of its feature RANSAC), on arbitrary arrays (no
+ * resident cloud needed): a is n_a x 33 floats, b is n_b x 33.  d^2(i, j) in fp32 without FMA, from 0.0f, over
+ * c = 0 .. 32 left to right: s = s + (a_c - b_c) * (a_c - b_c).  index[i] = the j of the lexicographically smallest
+ * (d^2, j) over the finite d^2 (a NaN or +inf never wins), sq_dist[i] = that d^2; a row with no finite d^2 gets -1 and
+ * +inf.  mutual != 0: index[i] becomes -1 unless the nearest a-row of b_{index[i]}, by the same rule, is i; sq_dist keeps
+ * the nearest d^2 either way.  0 <= n_a, n_b < 2^31; n_a = 0 does nothing; n_b = 0 gives all -1.  sq_dist may be NULL.
+ * a NULL a or index with n_a > 0, or b with n_a, n_b > 0 -> S4G_ERR_ARG; scratch the device cannot hold (8 bytes per
+ * row of a, and per row of b when mutual; the host form stages a, b and the outputs too) -> S4G_ERR_NOMEM.
+ * _dev: device buffers, enqueued on the context's stream, nothing synchronised.                                       */
+int s4g_fpfh_match(s4g_ctx* ctx, const float* a, int64_t n_a, const float* b, int64_t n_b, int mutual, int32_t* index,
+                   float* sq_dist);
+int s4g_fpfh_match_dev(s4g_ctx* ctx, const float* d_a, int64_t n_a, const float* d_b, int64_t n_b, int mutual,
+                       int32_t* d_index, float* d_sq_dist);
 /* Outlier removal on the resident sampled P.  j is the position in the array passed to s4g_set_cloud_p.  Both filters
  * write the kept j in ascending order to keep[0 .. *n_kept) (capacity nP; the output form of s4g_voxel_sample).
  *

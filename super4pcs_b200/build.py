@@ -12,7 +12,8 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "lib", "obj")
 LIB = os.path.join(HERE, "lib", "libs4g.so")
 SOURCES = ["context.cu", "verify.cu", "rigid.cu", "pairs.cu", "quads.cu", "sampler.cu", "comm.cu", "normals.cu", "outliers.cu",
-           "query.cu", "clusters.cu", "planes.cu", "voxel_grid.cu", "orient_normals.cu"]
+           "query.cu", "clusters.cu", "planes.cu", "voxel_grid.cu", "orient_normals.cu",
+           "fpfh.cu"]
 
 NVCC_FLAGS = [
     "-std=c++17", "-O3",

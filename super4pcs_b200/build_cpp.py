@@ -65,7 +65,8 @@ def build_all(force=False):
     inc = ["-I", os.path.join(ROOT, "include"), "-I", eig]
     srcs = [os.path.join(ROOT, "cpp", f) for f in ("match4pcsBase.cc", "super4pcs.cc", "pair_order.cc", "io.cc",
                                                       "normals.cc", "outliers.cc", "clusters.cc",
-                                                      "planes.cc", "voxel_grid.cc", "orient_normals.cc")]
+                                                      "planes.cc", "voxel_grid.cc", "orient_normals.cc",
+                                                      "features.cc")]
     link = ["-L", LIBDIR, "-ls4g", "-pthread", "-Wl,-rpath,$ORIGIN"]
     private = [os.path.join(ROOT, "cpp", f) for f in os.listdir(os.path.join(ROOT, "cpp")) if f.endswith(".h")]
     if force or _stale(lib, srcs + private + _headers() + [os.path.join(LIBDIR, "libs4g.so")]):

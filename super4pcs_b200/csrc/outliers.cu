@@ -222,6 +222,14 @@ int copy_keep(s4g_ctx* ctx, const FilterOut& o, int32_t* keep, int64_t* n_kept) 
 
 }  // namespace
 
+int s4g_launch_exclude_self(s4g_ctx* ctx, int32_t* d_exclude) {
+  S4G_CUDA(cudaSetDevice(ctx->device));
+  k_outlier_exclude<<<nblk(ctx->nP, 256), 256, 0, ctx->stream>>>(ctx->grid.pts, ctx->nP, d_exclude);
+  ctx->launches++;
+  S4G_CUDA(cudaGetLastError());
+  return S4G_OK;
+}
+
 extern "C" int s4g_statistical_outliers_dev(s4g_ctx* ctx, int k, double std_ratio, int32_t* d_keep, int64_t* d_n_kept,
                                             double* d_mean_dist, double* d_out2) {
   if (!ctx) return S4G_ERR_ARG;

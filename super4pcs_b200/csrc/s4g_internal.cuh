@@ -371,6 +371,9 @@ int s4g_launch_knn(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T, in
                    const int32_t* d_exclude, int32_t* d_index, float* d_sq_dist, unsigned long long* stats);
 // Enqueue the resident P points in the grid's sorted order as n x 3 queries (normals.cu): query t is GridDev::pts[t]
 int s4g_launch_sorted_queries(s4g_ctx* ctx, float* d_xyz);
+// Enqueue k_outlier_exclude over the resident P (outliers.cu): d_exclude[t] = the original index of sorted point t
+// (GridDev::pts[t].w), the exclusion list that makes query t of s4g_launch_sorted_queries skip its own point
+int s4g_launch_exclude_self(s4g_ctx* ctx, int32_t* d_exclude);
 // Enqueue k_radius_count over the resident P (query.cu): d_counts[j] = min(c_j, min_neighbors) (d_counts may be
 // nullptr), d_keep[j] = c_j >= min_neighbors, c_j the number of other P points with d^2 < sq_radius.  min_neighbors >= 1.
 int s4g_launch_radius_count(s4g_ctx* ctx, float sq_radius, int min_neighbors, int32_t* d_counts, uint8_t* d_keep);

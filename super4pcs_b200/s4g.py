@@ -113,6 +113,10 @@ def load_library():
         "s4g_normals_dev": ([vp, i32, f32, vp, vp, vp], i32),
         "s4g_orient_normals": ([vp, vp, i32, f32, vp, vp, vp, vp, vp], i32),
         "s4g_orient_normals_dev": ([vp, vp, i32, f32, vp, vp, vp, vp, vp], i32),
+        "s4g_fpfh": ([vp, vp, i32, f32, vp], i32),
+        "s4g_fpfh_dev": ([vp, vp, i32, f32, vp], i32),
+        "s4g_fpfh_match": ([vp, vp, C.c_int64, vp, C.c_int64, i32, vp, vp], i32),
+        "s4g_fpfh_match_dev": ([vp, vp, C.c_int64, vp, C.c_int64, i32, vp, vp], i32),
         "s4g_statistical_outliers": ([vp, i32, C.c_double, vp, vp, vp, vp], i32),
         "s4g_statistical_outliers_dev": ([vp, i32, C.c_double, vp, vp, vp, vp], i32),
         "s4g_radius_outliers": ([vp, f32, i32, vp, vp, vp], i32),
@@ -396,6 +400,39 @@ class Context:
         vp = None if viewpoint is None else _c(viewpoint).reshape(3)
         self._chk(self._L.s4g_orient_normals_dev(self.h, v(d_normals_ptr), int(k), float(sq_radius), _p(vp),
                                                  v(d_normals_out_ptr), v(d_root_ptr), v(d_out2_ptr), v(d_tree_edges_ptr)))
+
+    def fpfh(self, normals, k, sq_radius=np.inf):
+        """-> [nP, 33] float32: the FPFH descriptor of every resident P point (in the order of set_cloud_p) from its k
+        nearest other points within sq_radius and the normals (one row per point; (0, 0, 0) or non-finite = no normal,
+        which gives an all-zero descriptor).  Bins 0-10 f1, 11-21 f2, 22-32 f3.  Orient the normals consistently first:
+        their signs mirror f1 and f3.  1 <= k <= 64; see s4g.h (s4g_fpfh)."""
+        N = _c(normals).reshape(-1, 3)
+        if len(N) != self.nP:
+            raise ValueError("fpfh needs one normal per resident P point")
+        out = np.empty((self.nP, 33), _f)
+        self._chk(self._L.s4g_fpfh(self.h, _p(N), int(k), float(sq_radius), _p(out)))
+        return out
+
+    def fpfh_dev(self, d_normals_ptr, k, d_fpfh_ptr, sq_radius=np.inf):
+        """device pointers (nP x 3 float32 normals, nP x 33 float32 descriptors), stream-ordered, nothing synchronised"""
+        v = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        self._chk(self._L.s4g_fpfh_dev(self.h, v(d_normals_ptr), int(k), float(sq_radius), v(d_fpfh_ptr)))
+
+    def fpfh_match(self, a, b, mutual=False):
+        """-> (index [n_a] int32, sq_dist [n_a] float32): for every row of a (n_a x 33) the row of b (n_b x 33) with the
+        smallest (d^2, index), d^2 summed in fp32 over the 33 bins in order; -1 / +inf when no d^2 is finite.  mutual:
+        index[i] = -1 unless a[i] is also the nearest row of a to b[index[i]].  See s4g.h (s4g_fpfh_match)."""
+        A, B = _c(a).reshape(-1, 33), _c(b).reshape(-1, 33)
+        index, sq = np.empty(len(A), np.int32), np.empty(len(A), _f)
+        self._chk(self._L.s4g_fpfh_match(self.h, _p(A), len(A), _p(B), len(B), int(bool(mutual)), _p(index), _p(sq)))
+        return index, sq
+
+    def fpfh_match_dev(self, d_a_ptr, n_a, d_b_ptr, n_b, d_index_ptr, d_sq_dist_ptr=None, mutual=False):
+        """device pointers (n_a x 33 and n_b x 33 float32 descriptors, n_a int32 index, n_a float32 sq_dist or None),
+        stream-ordered, nothing synchronised"""
+        v = lambda p: C.c_void_p(p) if p else None  # noqa: E731
+        self._chk(self._L.s4g_fpfh_match_dev(self.h, v(d_a_ptr), int(n_a), v(d_b_ptr), int(n_b), int(bool(mutual)),
+                                             v(d_index_ptr), v(d_sq_dist_ptr)))
 
     def statistical_outliers(self, k, std_ratio):
         """-> (keep [n_kept] int32, mean_dist [nP] float64, mu, sigma): the resident P points (positions in the array of
