@@ -3,12 +3,10 @@
 
 #include <cmath>
 #include <cstdint>
-#include <cstdlib>
 #include <stdexcept>
-#include <string>
 
-#include "grid_delta.h"
 #include "s4g.h"
+#include "utils_context.h"
 
 namespace GlobalRegistration {
 namespace Utils {
@@ -21,26 +19,18 @@ std::vector<std::vector<int>> ExtractEuclideanClusters(const std::vector<Point3D
   std::vector<std::vector<int>> out;
   const std::size_t n = cloud.size();
   if (n == 0) return out;
-  std::vector<float> xyz(3 * n);
-  for (std::size_t i = 0; i < n; ++i)
-    for (int c = 0; c < 3; ++c) xyz[3 * i + c] = cloud[i].pos()[c];
+  const std::vector<float> xyz = internal::Positions(cloud);
   float delta = tolerance / 2.02f;
   if (!(delta > 0.f) || !std::isfinite(delta)) delta = internal::GridDelta(xyz, n, 16);
-  int device = 0;
-  if (const char* e = std::getenv("S4PCS_DEVICE")) device = std::atoi(e);
-  s4g_ctx* ctx = nullptr;
-  if (s4g_create(device, &ctx) != S4G_OK)
-    throw std::runtime_error("super4pcs-b200: ExtractEuclideanClusters: no CUDA device (there is no CPU fallback)");
   std::vector<int32_t> labels(n), members(n);
   std::vector<int64_t> offsets(n + 1);
   int64_t n_clusters = 0;
-  int rc = s4g_set_cloud_p(ctx, xyz.data(), int(n), delta);
-  if (rc == S4G_OK)
-    rc = s4g_euclidean_clusters(ctx, tolerance * tolerance, min_size, max_size, labels.data(), nullptr, &n_clusters,
-                                offsets.data(), members.data());
-  const std::string msg = rc == S4G_OK ? std::string() : std::string(s4g_error_string(ctx));
-  s4g_destroy(ctx);
-  if (rc != S4G_OK) throw std::runtime_error("super4pcs-b200: ExtractEuclideanClusters: " + msg);
+  internal::WithContext("ExtractEuclideanClusters", [&](s4g_ctx* ctx) {
+    const int rc = s4g_set_cloud_p(ctx, xyz.data(), int(n), delta);
+    return rc == S4G_OK ? s4g_euclidean_clusters(ctx, tolerance * tolerance, min_size, max_size, labels.data(), nullptr,
+                                                 &n_clusters, offsets.data(), members.data())
+                        : rc;
+  });
   out.resize(std::size_t(n_clusters));
   for (int64_t c = 0; c < n_clusters; ++c)
     out[std::size_t(c)].assign(members.begin() + offsets[c], members.begin() + offsets[c + 1]);

@@ -1,14 +1,11 @@
 // super4pcs-b200: Utils::EstimateNormals on top of s4g_normals (include/s4g.h).
 #include "super4pcs/utils/normals.h"
 
-#include <algorithm>
 #include <cmath>
-#include <cstdlib>
 #include <stdexcept>
-#include <string>
 
-#include "grid_delta.h"
 #include "s4g.h"
+#include "utils_context.h"
 
 namespace GlobalRegistration {
 namespace Utils {
@@ -19,23 +16,16 @@ int EstimateNormals(std::vector<Point3D>& cloud, int k, Point3D::Scalar max_dist
     throw std::runtime_error("super4pcs-b200: EstimateNormals: max_distance is negative or NaN");
   if (cloud.empty()) return 0;
   const std::size_t n = cloud.size();
-  std::vector<float> xyz(3 * n);
-  for (std::size_t i = 0; i < n; ++i)
-    for (int c = 0; c < 3; ++c) xyz[3 * i + c] = cloud[i].pos()[c];
-  int device = 0;
-  if (const char* e = std::getenv("S4PCS_DEVICE")) device = std::atoi(e);
-  s4g_ctx* ctx = nullptr;
-  if (s4g_create(device, &ctx) != S4G_OK)
-    throw std::runtime_error("super4pcs-b200: EstimateNormals: no CUDA device (there is no CPU fallback)");
+  const std::vector<float> xyz = internal::Positions(cloud);
   std::vector<float> normals(3 * n);
   const float vp[3] = {viewpoint ? (*viewpoint)[0] : 0.f, viewpoint ? (*viewpoint)[1] : 0.f,
                        viewpoint ? (*viewpoint)[2] : 0.f};
-  int rc = s4g_set_cloud_p(ctx, xyz.data(), int(n), internal::GridDelta(xyz, n, k));
-  if (rc == S4G_OK)
-    rc = s4g_normals(ctx, k, max_distance * max_distance, viewpoint ? vp : nullptr, normals.data(), nullptr);
-  const std::string msg = rc == S4G_OK ? std::string() : std::string(s4g_error_string(ctx));
-  s4g_destroy(ctx);
-  if (rc != S4G_OK) throw std::runtime_error("super4pcs-b200: EstimateNormals: " + msg);
+  internal::WithContext("EstimateNormals", [&](s4g_ctx* ctx) {
+    const int rc = s4g_set_cloud_p(ctx, xyz.data(), int(n), internal::GridDelta(xyz, n, k));
+    return rc == S4G_OK
+               ? s4g_normals(ctx, k, max_distance * max_distance, viewpoint ? vp : nullptr, normals.data(), nullptr)
+               : rc;
+  });
   int nonzero = 0;
   for (std::size_t i = 0; i < n; ++i) {
     const Point3D::VectorType v(normals[3 * i], normals[3 * i + 1], normals[3 * i + 2]);

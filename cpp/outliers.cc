@@ -4,42 +4,27 @@
 
 #include <cmath>
 #include <cstdint>
-#include <cstdlib>
 #include <stdexcept>
-#include <string>
 
-#include "grid_delta.h"
 #include "s4g.h"
+#include "utils_context.h"
 
 namespace GlobalRegistration {
 namespace Utils {
 
 namespace {
 
-std::vector<float> Positions(const std::vector<Point3D>& cloud) {
-  std::vector<float> xyz(3 * cloud.size());
-  for (std::size_t i = 0; i < cloud.size(); ++i)
-    for (int c = 0; c < 3; ++c) xyz[3 * i + c] = cloud[i].pos()[c];
-  return xyz;
-}
-
 // runs filter(ctx, keep, &n_kept) on a short-lived context holding the cloud with grid delta `delta`, then keeps the
 // points keep[0 .. n_kept) (ascending) in place; returns how many were removed
 template <class Filter>
 int Apply(std::vector<Point3D>& cloud, const std::vector<float>& xyz, float delta, const char* who, Filter filter) {
   const std::size_t n = cloud.size();
-  int device = 0;
-  if (const char* e = std::getenv("S4PCS_DEVICE")) device = std::atoi(e);
-  s4g_ctx* ctx = nullptr;
-  if (s4g_create(device, &ctx) != S4G_OK)
-    throw std::runtime_error(std::string("super4pcs-b200: ") + who + ": no CUDA device (there is no CPU fallback)");
   std::vector<int32_t> keep(n);
   int64_t n_kept = 0;
-  int rc = s4g_set_cloud_p(ctx, xyz.data(), int(n), delta);
-  if (rc == S4G_OK) rc = filter(ctx, keep.data(), &n_kept);
-  const std::string msg = rc == S4G_OK ? std::string() : std::string(s4g_error_string(ctx));
-  s4g_destroy(ctx);
-  if (rc != S4G_OK) throw std::runtime_error(std::string("super4pcs-b200: ") + who + ": " + msg);
+  internal::WithContext(who, [&](s4g_ctx* ctx) {
+    const int rc = s4g_set_cloud_p(ctx, xyz.data(), int(n), delta);
+    return rc == S4G_OK ? filter(ctx, keep.data(), &n_kept) : rc;
+  });
   for (int64_t s = 0; s < n_kept; ++s)
     if (keep[s] != s) cloud[s] = cloud[keep[s]];   // keep[s] >= s: ascending, so no survivor is overwritten first
   cloud.resize(std::size_t(n_kept));
@@ -50,7 +35,7 @@ int Apply(std::vector<Point3D>& cloud, const std::vector<float>& xyz, float delt
 
 int RemoveStatisticalOutliers(std::vector<Point3D>& cloud, int k, double std_ratio) {
   if (cloud.empty()) return 0;
-  const std::vector<float> xyz = Positions(cloud);
+  const std::vector<float> xyz = internal::Positions(cloud);
   return Apply(cloud, xyz, internal::GridDelta(xyz, cloud.size(), k), "RemoveStatisticalOutliers",
                [&](s4g_ctx* ctx, int32_t* keep, int64_t* n_kept) {
                  return s4g_statistical_outliers(ctx, k, std_ratio, keep, n_kept, nullptr, nullptr);
@@ -61,7 +46,7 @@ int RemoveRadiusOutliers(std::vector<Point3D>& cloud, Point3D::Scalar radius, in
   if (std::isnan(radius) || radius < 0)
     throw std::runtime_error("super4pcs-b200: RemoveRadiusOutliers: radius is negative or NaN");
   if (cloud.empty()) return 0;
-  const std::vector<float> xyz = Positions(cloud);
+  const std::vector<float> xyz = internal::Positions(cloud);
   float delta = radius / 2.02f;
   if (!(delta > 0.f) || !std::isfinite(delta)) delta = internal::GridDelta(xyz, cloud.size(), min_neighbors);
   return Apply(cloud, xyz, delta, "RemoveRadiusOutliers", [&](s4g_ctx* ctx, int32_t* keep, int64_t* n_kept) {

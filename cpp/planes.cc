@@ -3,12 +3,10 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstdlib>
 #include <stdexcept>
-#include <string>
 
-#include "grid_delta.h"
 #include "s4g.h"
+#include "utils_context.h"
 
 namespace GlobalRegistration {
 namespace Utils {
@@ -22,27 +20,20 @@ std::vector<PlaneModel> SegmentPlanes(const std::vector<Point3D>& cloud, Point3D
   std::vector<PlaneModel> out;
   const std::size_t n = cloud.size();
   if (n == 0) return out;
-  std::vector<float> xyz(3 * n);
-  for (std::size_t i = 0; i < n; ++i)
-    for (int c = 0; c < 3; ++c) xyz[3 * i + c] = cloud[i].pos()[c];
-  int device = 0;
-  if (const char* e = std::getenv("S4PCS_DEVICE")) device = std::atoi(e);
-  s4g_ctx* ctx = nullptr;
-  if (s4g_create(device, &ctx) != S4G_OK)
-    throw std::runtime_error("super4pcs-b200: SegmentPlanes: no CUDA device (there is no CPU fallback)");
+  const std::vector<float> xyz = internal::Positions(cloud);
   // at most n planes are accepted (each claims a point), so the outputs never need more rows than that
   const int rows = int(std::min<std::size_t>(std::size_t(max_planes), n));
   std::vector<int32_t> labels(n), members(n);
   std::vector<int64_t> offsets(std::size_t(rows) + 1);
   std::vector<s4g_plane> planes{std::size_t(rows)};
   int n_planes = 0;
-  int rc = s4g_set_cloud_p(ctx, xyz.data(), int(n), internal::GridDelta(xyz, n, 16));
-  if (rc == S4G_OK)
-    rc = s4g_segment_planes(ctx, threshold, iterations, seed, refine ? 1 : 0, rows, min_inliers, labels.data(),
-                            planes.data(), &n_planes, offsets.data(), members.data(), nullptr);
-  const std::string msg = rc == S4G_OK ? std::string() : std::string(s4g_error_string(ctx));
-  s4g_destroy(ctx);
-  if (rc != S4G_OK) throw std::runtime_error("super4pcs-b200: SegmentPlanes: " + msg);
+  internal::WithContext("SegmentPlanes", [&](s4g_ctx* ctx) {
+    const int rc = s4g_set_cloud_p(ctx, xyz.data(), int(n), internal::GridDelta(xyz, n, 16));
+    return rc == S4G_OK ? s4g_segment_planes(ctx, threshold, iterations, seed, refine ? 1 : 0, rows, min_inliers,
+                                             labels.data(), planes.data(), &n_planes, offsets.data(), members.data(),
+                                             nullptr)
+                        : rc;
+  });
   out.resize(std::size_t(n_planes));
   for (int r = 0; r < n_planes; ++r) {
     for (int c = 0; c < 4; ++c) out[std::size_t(r)].coefficients[std::size_t(c)] = planes[std::size_t(r)].coefficients[c];

@@ -3,11 +3,10 @@
 
 #include <cmath>
 #include <cstdint>
-#include <cstdlib>
 #include <stdexcept>
-#include <string>
 
 #include "s4g.h"
+#include "utils_context.h"
 
 namespace GlobalRegistration {
 namespace Utils {
@@ -30,18 +29,12 @@ int VoxelGridFilter(std::vector<Point3D>& cloud, Point3D::Scalar leaf, int min_p
       if (colour) rgb[3 * i + c] = cloud[i].rgb()[c];
     }
   std::vector<float> xyz_out(3 * n), nrm_out(3 * n), rgb_out(colour ? 3 * n : 0);
-  int device = 0;
-  if (const char* e = std::getenv("S4PCS_DEVICE")) device = std::atoi(e);
-  s4g_ctx* ctx = nullptr;
-  if (s4g_create(device, &ctx) != S4G_OK)
-    throw std::runtime_error("super4pcs-b200: VoxelGridFilter: no CUDA device (there is no CPU fallback)");
   int64_t m = 0;
-  const int rc = s4g_voxel_grid(ctx, xyz.data(), nrm.data(), colour ? rgb.data() : nullptr, int64_t(n), leaf, min_points,
-                                xyz_out.data(), nrm_out.data(), colour ? rgb_out.data() : nullptr, nullptr, nullptr,
-                                nullptr, &m);
-  const std::string msg = rc == S4G_OK ? std::string() : std::string(s4g_error_string(ctx));
-  s4g_destroy(ctx);
-  if (rc != S4G_OK) throw std::runtime_error("super4pcs-b200: VoxelGridFilter: " + msg);
+  internal::WithContext("VoxelGridFilter", [&](s4g_ctx* ctx) {
+    return s4g_voxel_grid(ctx, xyz.data(), nrm.data(), colour ? rgb.data() : nullptr, int64_t(n), leaf, min_points,
+                          xyz_out.data(), nrm_out.data(), colour ? rgb_out.data() : nullptr, nullptr, nullptr, nullptr,
+                          &m);
+  });
   std::vector<Point3D> out(static_cast<std::size_t>(m));
   for (std::size_t v = 0; v < out.size(); ++v) {
     out[v] = Point3D(xyz_out[3 * v], xyz_out[3 * v + 1], xyz_out[3 * v + 2]);

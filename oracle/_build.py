@@ -1,5 +1,7 @@
 """TEST INFRASTRUCTURE ONLY: builds oracle/liboracle_port.so and, when the reference is present,
-oracle/_ref/liboracle_ref.so (see oracle/Makefile) and the staged copy oracle/_ref/reference (stage_reference)."""
+oracle/_ref/liboracle_ref.so (see oracle/Makefile) and the staged copy oracle/_ref/reference (stage_reference); the
+restatements of the point-cloud utilities (port_lib) and their reference-side libraries (ref_lib)."""
+import ctypes as C
 import os
 import shutil
 import subprocess
@@ -44,6 +46,91 @@ def _stale(target, sources):
     return any(os.path.exists(s) and os.path.getmtime(s) > t for s in sources)
 
 
+def _env():
+    """the environment of every compiler call here: g++ itself, whatever CXX and CC name"""
+    env = dict(os.environ)
+    env.pop("CXX", None)
+    env.pop("CC", None)
+    return env
+
+
+_libs = {}
+
+
+def _lib(path):
+    if path not in _libs:
+        _libs[path] = C.CDLL(path)
+    return _libs[path]
+
+
+def _p(a):
+    return None if a is None else a.ctypes.data_as(C.c_void_p)
+
+
+def eigen_root():
+    """the Eigen that code compiled against include/super4pcs/ needs: S4_EIGEN_ROOT, the reference's copy or the
+    system's; None when there is none"""
+    for c in (os.environ.get("S4_EIGEN_ROOT"), os.path.join(REFERENCE_ROOT, "3rdparty", "Eigen"),
+              "/usr/include/eigen3"):
+        if c and os.path.exists(os.path.join(c, "Eigen", "Core")):
+            return c
+    return None
+
+
+_PORT_FLAGS = ("-std=c++11", "-O2", "-ffp-contract=off", "-fopenmp")
+# the restatements of the point-cloud utilities: name -> (compile flags, the ports besides oracle/<name>_port.cc that
+# its library holds).  tests/build_shim.py compiles each oracle/<name>_port.cc into the CPU stand-in with these flags.
+PORTS = {
+    "nearest": (_PORT_FLAGS, ()),
+    "nearest_any": (_PORT_FLAGS, ()),
+    "range": (_PORT_FLAGS, ()),
+    "knn": (_PORT_FLAGS, ()),
+    "normals": (_PORT_FLAGS, ("knn",)),
+    "orient_normals": (_PORT_FLAGS, ("knn",)),
+    "outliers": (_PORT_FLAGS, ("knn",)),
+    "clusters": (_PORT_FLAGS, ()),
+    # -O3: the CPU baseline of scripts/planes_bench.py
+    "planes": (("-std=c++11", "-O3", "-ffp-contract=off", "-fopenmp"), ()),
+    # one thread, although the source has an OpenMP pragma: the CPU baseline of scripts/voxel_grid_bench.py
+    "voxel_grid": (("-std=c++11", "-O2", "-ffp-contract=off"), ()),
+    "fpfh": (("-std=c++17", "-O2", "-ffp-contract=off", "-fopenmp"), ("knn",)),  # C++17 for its hex-float literals
+}
+
+
+def port_src(name):
+    return os.path.join(HERE, name + "_port.cc")
+
+
+def port_lib(name, force=False):
+    """oracle/liboracle_<name>.so, the restatement PORTS[name], rebuilt when it is older than its sources"""
+    flags, others = PORTS[name]
+    srcs = [port_src(n) for n in (name,) + others]
+    so = os.path.join(HERE, "liboracle_%s.so" % name)
+    if force or _stale(so, srcs):
+        subprocess.check_call(["g++", *flags, "-fPIC", "-shared", *srcs, "-o", so], env=_env())
+    return so
+
+
+# the queries whose reference side is the reference's own kd-tree, in oracle/<name>_ref.cc
+REF_LIBS = ("nearest", "nearest_any", "range")
+
+
+def ref_lib(name, force=False):
+    """oracle/_ref/liboracle_ref_<name>.so (oracle/<name>_ref.cc linked against build_ref()'s library), or None when it
+    can be neither built (no reference sources) nor found"""
+    src = os.path.join(HERE, name + "_ref.cc")
+    so = os.path.join(HERE, "_ref", "liboracle_ref_%s.so" % name)
+    ref = REFERENCE_ROOT
+    base = build_ref()
+    if base is not None and os.path.isdir(os.path.join(ref, "src", "super4pcs")) and (force or _stale(so, [src, base])):
+        # the flags of oracle/Makefile's reference build (the reference's Release configuration)
+        subprocess.check_call(["g++", "-std=c++11", "-O3", "-DNDEBUG", "-fopenmp", "-DSUPER4PCS_USE_OPENMP",
+                               "-DEIGEN_DONT_PARALLELIZE", "-I", os.path.join(ref, "src"),
+                               "-I", os.path.join(ref, "3rdparty", "Eigen"), "-fPIC", "-w", "-shared", src,
+                               "-o", so, "-L", os.path.dirname(base), "-loracle_ref", "-Wl,-rpath,$ORIGIN"], env=_env())
+    return so if os.path.exists(so) else None
+
+
 def build_port(force=False):
     if force or _stale(PORT_SO, [os.path.join(HERE, "port.cc")]):
         subprocess.check_call(["make", "-C", HERE, "port"], stdout=subprocess.DEVNULL)
@@ -72,18 +159,11 @@ def build_dropin_harness(force=False):
     root = os.path.dirname(HERE)
     libdir = os.path.join(root, "super4pcs_b200", "lib")
     prod = os.path.join(libdir, "libsuper4pcs_b200.so")
-    eig = None
-    for c in (os.environ.get("S4_EIGEN_ROOT"), os.path.join(REFERENCE_ROOT, "3rdparty", "Eigen"), "/usr/include/eigen3"):
-        if c and os.path.exists(os.path.join(c, "Eigen", "Core")):
-            eig = c
-            break
+    eig = eigen_root()
     src = os.path.join(HERE, "ref_harness.cc")
     if eig and os.path.exists(prod) and (force or _stale(DROPIN_SO, [src, prod])):
         os.makedirs(os.path.dirname(DROPIN_SO), exist_ok=True)
-        env = dict(os.environ)
-        env.pop("CXX", None)
-        env.pop("CC", None)
         subprocess.check_call(["g++", "-std=c++14", "-O3", "-DNDEBUG", "-fPIC", "-w", "-fopenmp", "-DSUPER4PCS_USE_OPENMP",
                                "-shared", "-I", os.path.join(root, "include"), "-I", eig, src, "-o", DROPIN_SO,
-                               "-L", libdir, "-lsuper4pcs_b200", "-ls4g", "-Wl,-rpath,$ORIGIN/../../super4pcs_b200/lib"], env=env)
+                               "-L", libdir, "-lsuper4pcs_b200", "-ls4g", "-Wl,-rpath,$ORIGIN/../../super4pcs_b200/lib"], env=_env())
     return DROPIN_SO if os.path.exists(DROPIN_SO) else None

@@ -10,33 +10,17 @@
 
 The reference has no clustering; its kd-tree's range query (oracle.range.RefRange) is the reference side of the graph."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
 from . import _build
-from .nearest import _env, _lib, _p
+from ._build import _lib, _p
 
-HERE = _build.HERE
-PORT_SRC = os.path.join(HERE, "clusters_port.cc")
-PORT_SO = os.path.join(HERE, "liboracle_clusters.so")
 _f = np.float32
 
 
-def build_port(force=False):
-    if force or _build._stale(PORT_SO, [PORT_SRC]):
-        subprocess.check_call(["g++", "-std=c++11", "-O2", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared", PORT_SRC,
-                               "-o", PORT_SO], env=_env())
-    return PORT_SO
-
-
-def build():
-    build_port()
-
-
 def _L():
-    L = _lib(build_port())
+    L = _lib(_build.port_lib("clusters"))
     L.clusters_root_bruteforce.argtypes = [C.c_void_p, C.c_long, C.c_float, C.c_void_p]
     L.clusters_root_from_lists.argtypes = [C.c_long, C.c_void_p, C.c_void_p, C.c_void_p]
     L.clusters_finish.argtypes = [C.c_long, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]

@@ -9,17 +9,12 @@ neighbourhoods and the nearest descriptor.
 
 The reference computes no descriptors, so there is no reference-side library."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
 from . import _build
-from .nearest import _env, _lib, _p
+from ._build import _lib, _p
 
-HERE = _build.HERE
-PORT_SRCS = [os.path.join(HERE, "fpfh_port.cc"), os.path.join(HERE, "knn_port.cc")]
-PORT_SO = os.path.join(HERE, "liboracle_fpfh.so")
 _f = np.float32
 
 
@@ -27,19 +22,8 @@ class FPFHError(ValueError):
     """the port's S4G_ERR_ARG"""
 
 
-def build_port(force=False):
-    if force or _build._stale(PORT_SO, PORT_SRCS):
-        subprocess.check_call(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared", *PORT_SRCS,
-                               "-o", PORT_SO], env=_env())
-    return PORT_SO
-
-
-def build():
-    build_port()
-
-
 def _L():
-    L = _lib(build_port())
+    L = _lib(_build.port_lib("fpfh"))
     L.fpfh_port.argtypes = [C.c_void_p, C.c_long, C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p,
                             C.c_void_p]
     L.fpfh_port.restype = C.c_int

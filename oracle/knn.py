@@ -9,34 +9,18 @@ points.
 The reference's kd-tree has no k-nearest query, so there is no reference-side library here: the reference side reuses
 oracle.range.RefRange and oracle.nearest_any.RefNearestAny."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
 from . import _build
-from .nearest import _env, _lib, _p
+from ._build import _lib, _p
 
-HERE = _build.HERE
-PORT_SRC = os.path.join(HERE, "knn_port.cc")
-PORT_SO = os.path.join(HERE, "liboracle_knn.so")
 _f = np.float32
-
-
-def build_port(force=False):
-    if force or _build._stale(PORT_SO, [PORT_SRC]):
-        subprocess.check_call(["g++", "-std=c++11", "-O2", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared", PORT_SRC,
-                               "-o", PORT_SO], env=_env())
-    return PORT_SO
-
-
-def build():
-    build_port()
 
 
 def bruteforce(P, X, k, sq_radius=np.inf, T16=None, exclude=None):
     """-> (index [n, k] int32, sq_dist [n, k] float32): the s4g_knn contract over all of P"""
-    L = _lib(build_port())
+    L = _lib(_build.port_lib("knn"))
     L.knn_bruteforce.argtypes = [C.c_void_p, C.c_long, C.c_void_p, C.c_long, C.c_void_p, C.c_int, C.c_float, C.c_void_p,
                                  C.c_void_p, C.c_void_p]
     P, X = np.ascontiguousarray(P, _f).reshape(-1, 3), np.ascontiguousarray(X, _f).reshape(-1, 3)

@@ -6,35 +6,19 @@
 
 The reference has no normal estimation (its kd-tree has no k-nearest query), so there is no reference-side library."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
 from . import _build
-from .nearest import _env, _lib, _p
+from ._build import _lib, _p
 
-HERE = _build.HERE
-PORT_SRCS = [os.path.join(HERE, "normals_port.cc"), os.path.join(HERE, "knn_port.cc")]
-PORT_SO = os.path.join(HERE, "liboracle_normals.so")
 _f = np.float32
-
-
-def build_port(force=False):
-    if force or _build._stale(PORT_SO, PORT_SRCS):
-        subprocess.check_call(["g++", "-std=c++11", "-O2", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared", *PORT_SRCS,
-                               "-o", PORT_SO], env=_env())
-    return PORT_SO
-
-
-def build():
-    build_port()
 
 
 def port(P, k, sq_radius=np.inf, viewpoint=None, which=None, rows=False):
     """-> (normals [n, 3], eigenvalues [n, 3]) float32 of the P points `which` (default all, n = len(P)); rows=True: also
     their knn rows [n, k] int32"""
-    L = _lib(build_port())
+    L = _lib(_build.port_lib("normals"))
     L.normals_port.argtypes = [C.c_void_p, C.c_long, C.c_void_p, C.c_long, C.c_int, C.c_float, C.c_void_p, C.c_void_p,
                                C.c_void_p, C.c_void_p]
     P = np.ascontiguousarray(P, _f).reshape(-1, 3)

@@ -8,17 +8,12 @@ minimum spanning forest of the k-nearest graph.
 
 The reference has no normal estimation, so there is no reference-side library."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
 from . import _build
-from .nearest import _env, _lib, _p
+from ._build import _lib, _p
 
-HERE = _build.HERE
-PORT_SRCS = [os.path.join(HERE, "orient_normals_port.cc"), os.path.join(HERE, "knn_port.cc")]
-PORT_SO = os.path.join(HERE, "liboracle_orient_normals.so")
 _f = np.float32
 
 
@@ -26,22 +21,11 @@ class OrientError(ValueError):
     """the port's S4G_ERR_ARG: bad arguments or a non-finite normal component"""
 
 
-def build_port(force=False):
-    if force or _build._stale(PORT_SO, PORT_SRCS):
-        subprocess.check_call(["g++", "-std=c++11", "-O2", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared", *PORT_SRCS,
-                               "-o", PORT_SO], env=_env())
-    return PORT_SO
-
-
-def build():
-    build_port()
-
-
 def port(P, normals, k, sq_radius=np.inf, viewpoint=None, rows=None, out=None):
     """-> (oriented [n, 3] float32, root [n] int32, n_components, tree_edges [n_tree, 2] int32), Context.orient_normals'
     form.  rows: [n, k] int32 knn rows with self-exclusion to use instead of the brute force.  out: the array to write the
     oriented normals to (may be `normals` itself: in place).  Raises OrientError where the contract gives S4G_ERR_ARG."""
-    L = _lib(build_port())
+    L = _lib(_build.port_lib("orient_normals"))
     L.orient_normals_port.argtypes = [C.c_void_p, C.c_long, C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.orient_normals_port.restype = C.c_int

@@ -9,33 +9,17 @@
 The reference has no outlier removal; its kd-tree's range query (oracle.range.RefRange) is the reference side of the
 radius filter's counts."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
 from . import _build
-from .nearest import _env, _lib, _p
+from ._build import _lib, _p
 
-HERE = _build.HERE
-PORT_SRCS = [os.path.join(HERE, "outliers_port.cc"), os.path.join(HERE, "knn_port.cc")]
-PORT_SO = os.path.join(HERE, "liboracle_outliers.so")
 _f = np.float32
 
 
-def build_port(force=False):
-    if force or _build._stale(PORT_SO, PORT_SRCS):
-        subprocess.check_call(["g++", "-std=c++11", "-O2", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared", *PORT_SRCS,
-                               "-o", PORT_SO], env=_env())
-    return PORT_SO
-
-
-def build():
-    build_port()
-
-
 def _L():
-    L = _lib(build_port())
+    L = _lib(_build.port_lib("outliers"))
     L.outlier_mean_rows.argtypes = [C.c_void_p, C.c_long, C.c_void_p, C.c_long, C.c_int, C.c_void_p]
     L.outlier_moments.argtypes = [C.c_void_p, C.c_long, C.c_void_p]
     L.outlier_flags.argtypes = [C.c_void_p, C.c_long, C.c_void_p, C.c_double, C.c_void_p]

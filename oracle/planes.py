@@ -8,17 +8,12 @@
 
 The reference has no plane segmentation, so there is no reference side."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
 from . import _build
-from .nearest import _env, _lib, _p
+from ._build import _lib, _p
 
-HERE = _build.HERE
-PORT_SRC = os.path.join(HERE, "planes_port.cc")
-PORT_SO = os.path.join(HERE, "liboracle_planes.so")
 _f = np.float32
 
 # s4g_plane (include/s4g.h), as super4pcs_b200.s4g.PLANE_DTYPE
@@ -26,19 +21,8 @@ PLANE_DTYPE = np.dtype([("coefficients", np.float32, 4), ("hypothesis", np.float
                         ("sample", np.int32, 3), ("hypothesis_inliers", np.int64), ("n_inliers", np.int64)])
 
 
-def build_port(force=False):
-    if force or _build._stale(PORT_SO, [PORT_SRC]):
-        subprocess.check_call(["g++", "-std=c++11", "-O3", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared", PORT_SRC,
-                               "-o", PORT_SO], env=_env())
-    return PORT_SO
-
-
-def build():
-    build_port()
-
-
 def _L():
-    L = _lib(build_port())
+    L = _lib(_build.port_lib("planes"))
     L.planes_hypotheses.argtypes = [C.c_void_p, C.c_void_p, C.c_long, C.c_long, C.c_uint64, C.c_void_p, C.c_void_p,
                                     C.c_void_p]
     L.planes_counts.argtypes = [C.c_void_p, C.c_void_p, C.c_long, C.c_long, C.c_void_p, C.c_float, C.c_void_p]

@@ -8,56 +8,22 @@ P point closer than a radius to any query point.
 
 Both return CSR lists: (offsets [n + 1] int64, index [total] int32, sq_dist [total] float32)."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
 from . import _build
-from .nearest import _env, _lib, _p
+from ._build import _lib, _p
 
-HERE = _build.HERE
-PORT_SRC = os.path.join(HERE, "range_port.cc")
-PORT_SO = os.path.join(HERE, "liboracle_range.so")
-REF_SRC = os.path.join(HERE, "range_ref.cc")
-REF_SO = os.path.join(HERE, "_ref", "liboracle_ref_range.so")
 _f = np.float32
 
 
-def build_port(force=False):
-    if force or _build._stale(PORT_SO, [PORT_SRC]):
-        subprocess.check_call(["g++", "-std=c++11", "-O2", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared", PORT_SRC,
-                               "-o", PORT_SO], env=_env())
-    return PORT_SO
-
-
-def build_ref(force=False):
-    """the path of the reference-side library, or None when it can be neither built (no reference sources) nor found"""
-    ref = _build.REFERENCE_ROOT
-    base = _build.build_ref()
-    if base is not None and os.path.isdir(os.path.join(ref, "src", "super4pcs")) and \
-            (force or _build._stale(REF_SO, [REF_SRC, base])):
-        # the flags of oracle/Makefile's reference build (the reference's Release configuration)
-        subprocess.check_call(["g++", "-std=c++11", "-O3", "-DNDEBUG", "-fopenmp", "-DSUPER4PCS_USE_OPENMP",
-                               "-DEIGEN_DONT_PARALLELIZE", "-I", os.path.join(ref, "src"),
-                               "-I", os.path.join(ref, "3rdparty", "Eigen"), "-fPIC", "-w", "-shared", REF_SRC,
-                               "-o", REF_SO, "-L", os.path.dirname(base), "-loracle_ref", "-Wl,-rpath,$ORIGIN"],
-                              env=_env())
-    return REF_SO if os.path.exists(REF_SO) else None
-
-
-def build():
-    build_port()
-    build_ref()
-
-
 def ref_available():
-    return build_ref() is not None
+    return _build.ref_lib("range") is not None
 
 
 def bruteforce(P, X, sq_radius, T16=None):
     """-> (offsets, index, sq_dist): the s4g_range contract over all of P"""
-    L = _lib(build_port())
+    L = _lib(_build.port_lib("range"))
     args = [C.c_void_p, C.c_long, C.c_void_p, C.c_long, C.c_void_p, C.c_float]
     L.range_bruteforce_count.argtypes = args + [C.c_void_p]
     L.range_bruteforce_fill.argtypes = args + [C.c_void_p, C.c_void_p, C.c_void_p]
@@ -76,9 +42,10 @@ class RefRange:
     configureOverlap(overlap)."""
 
     def __init__(self, P, Q, delta, overlap=1.0, sample_size=0):
-        path = build_ref()
+        path = _build.ref_lib("range")
         if path is None:
-            raise RuntimeError("reference oracle not available (no reference sources and no prebuilt %s)" % REF_SO)
+            raise RuntimeError("reference oracle not available (no reference sources and no prebuilt "
+                               "oracle/_ref/liboracle_ref_range.so)")
         L = self._L = _lib(path)
         L.range_ref_create.restype = C.c_void_p
         L.range_ref_create.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_float, C.c_float, C.c_long]

@@ -1,22 +1,17 @@
 """TEST INFRASTRUCTURE ONLY: the oracle of s4g_voxel_grid (include/s4g.h).
 
-* `port` -- oracle/libvoxel_grid_port.so (oracle/voxel_grid_port.cc): the contract restated operation for operation, so
+* `port` -- oracle/liboracle_voxel_grid.so (oracle/voxel_grid_port.cc): the contract restated operation for operation, so
             that it equals the device bit for bit.
 
 The reference has no voxel-grid filter; its UniformDistSampler (s4g_voxel_sample) keeps the first point of the same
 voxels, which is the `first` output at min_points = 1."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
 from . import _build
-from .nearest import _env, _lib, _p
+from ._build import _lib, _p
 
-HERE = _build.HERE
-PORT_SRCS = [os.path.join(HERE, "voxel_grid_port.cc")]
-PORT_SO = os.path.join(HERE, "libvoxel_grid_port.so")
 _f = np.float32
 
 
@@ -24,19 +19,8 @@ class VoxelGridError(ValueError):
     """the port's S4G_ERR_ARG: bad arguments, a non-finite or out-of-range coordinate, or too wide a span"""
 
 
-def build_port(force=False):
-    if force or _build._stale(PORT_SO, PORT_SRCS):
-        subprocess.check_call(["g++", "-std=c++11", "-O2", "-ffp-contract=off", "-fPIC", "-shared", *PORT_SRCS,
-                               "-o", PORT_SO], env=_env())
-    return PORT_SO
-
-
-def build():
-    build_port()
-
-
 def _L():
-    L = _lib(build_port())
+    L = _lib(_build.port_lib("voxel_grid"))
     L.voxel_grid_port.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_long, C.c_float, C.c_int] + [C.c_void_p] * 7
     L.voxel_grid_port.restype = C.c_int
     return L

@@ -1,5 +1,4 @@
-// TEST INFRASTRUCTURE ONLY (oracle/voxel_grid.py and tests/stubs/s4g_voxel_grid_shim.cc build it; never linked into the
-// product).
+// TEST INFRASTRUCTURE ONLY (oracle/_build.py and tests/build_shim.py build it; never linked into the product).
 //
 // Plain restatement of s4g_voxel_grid (include/s4g.h), operation for operation:
 //   s = 1.0f / leaf; the voxel of point i is (floor(fl(x s)), floor(fl(y s)), floor(fl(z s))); a floor that is NaN or

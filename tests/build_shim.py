@@ -1,6 +1,7 @@
 """TEST INFRASTRUCTURE ONLY: builds tests/_build/libs4g_oracle_shim.so (tests/stubs/s4g_oracle_shim.cc), a
-stand-in for libs4g.so answered by the CPU oracle, used through LD_PRELOAD by tests/test_host_logic_cpu.py to run the
-host logic of the C++ layer without a GPU.  Never part of the product."""
+stand-in for libs4g.so answered by the CPU oracle, used through LD_PRELOAD by the CPU tests of the C++ layer to run its
+host logic without a GPU.  The restatements of the point-cloud utilities (oracle/<name>_port.cc) are compiled into it,
+each with the flags of its oracle library.  Never part of the product."""
 import os
 import subprocess
 
@@ -13,15 +14,18 @@ def build(force=False):
     from oracle import _build
     port = _build.build_port()
     src = os.path.join(HERE, "stubs", "s4g_oracle_shim.cc")
-    deps = [src, port, os.path.join(ROOT, "include", "s4g.h")]
-    if force or not os.path.exists(OUT) or any(os.path.getmtime(d) > os.path.getmtime(OUT) for d in deps):
+    ports = {name: _build.port_src(name) for name in _build.PORTS}
+    deps = [src, port, os.path.join(ROOT, "include", "s4g.h"), *ports.values()]
+    if force or _build._stale(OUT, deps):
         os.makedirs(os.path.dirname(OUT), exist_ok=True)
-        env = dict(os.environ)
-        env.pop("CXX", None)
-        env.pop("CC", None)
-        subprocess.check_call(["g++", "-std=c++14", "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-I", os.path.join(ROOT, "include"),
-                               src, "-o", OUT, "-L", os.path.dirname(port), "-loracle_port",
-                               "-Wl,-rpath," + os.path.dirname(port)], env=env)
+        objs = []
+        for name, cc in ports.items():
+            objs.append(os.path.join(os.path.dirname(OUT), name + "_port.o"))
+            subprocess.check_call(["g++", *_build.PORTS[name][0], "-fPIC", "-c", cc, "-o", objs[-1]], env=_build._env())
+        subprocess.check_call(["g++", "-std=c++14", "-O2", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
+                               "-I", os.path.join(ROOT, "include"), src, *objs, "-o", OUT,
+                               "-L", os.path.dirname(port), "-loracle_port", "-Wl,-rpath," + os.path.dirname(port)],
+                              env=_build._env())
     return OUT
 
 

@@ -1,62 +1,22 @@
 """Builds and runs tests/cpp/clusters_main.cc, the test program of Utils::ExtractEuclideanClusters, for
-tests/test_clusters_cpu.py (on the oracle stand-in) and tests/test_clusters_gpu.py (on the real library), and the
-stand-in's companion that answers s4g_euclidean_clusters on the CPU (tests/stubs/s4g_clusters_shim.cc).  Also the grid
+tests/test_clusters_cpu.py (on the oracle stand-in) and tests/test_clusters_gpu.py (on the real library).  Also the grid
 delta rule of the function, and clouds whose clusters are known."""
-import os
-import subprocess
-
 import numpy as np
 
-from tests import knn as tknn, normals as tnormals
+from tests import cpp_main, normals as tnormals
 
-ROOT = tknn.ROOT
 _f = np.float32
 
 
 def build(outdir):
-    """compiles the program into `outdir` against the C++ layer; None when the layer or Eigen is missing"""
-    from oracle import _build
-    from super4pcs_b200 import build_cpp
-    if build_cpp.build_all()["lib"] is None:
-        return None
-    eig = None
-    for c in (os.environ.get("S4_EIGEN_ROOT"), os.path.join(_build.REFERENCE_ROOT, "3rdparty", "Eigen"), "/usr/include/eigen3"):
-        if c and os.path.exists(os.path.join(c, "Eigen", "Core")):
-            eig = c
-            break
-    if eig is None:
-        return None
-    libdir = os.path.join(ROOT, "super4pcs_b200", "lib")
-    exe = os.path.join(str(outdir), "clusters_main")
-    subprocess.check_call(["g++", "-std=c++14", "-O2", "-w", "-I", os.path.join(ROOT, "include"), "-I", eig,
-                           os.path.join(ROOT, "tests", "cpp", "clusters_main.cc"), "-o", exe, "-L", libdir,
-                           "-lsuper4pcs_b200", "-ls4g", "-Wl,-rpath," + libdir], env=tknn._env())
-    return exe
-
-
-def build_shim(outdir):
-    """compiles tests/stubs/s4g_clusters_shim.cc (+ oracle/clusters_port.cc) into `outdir`; preload it ahead of the
-    oracle stand-in of libs4g"""
-    out = os.path.join(str(outdir), "libs4g_clusters_shim.so")
-    subprocess.check_call(["g++", "-std=c++14", "-O2", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
-                           "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "stubs", "s4g_clusters_shim.cc"),
-                           os.path.join(ROOT, "oracle", "clusters_port.cc"), "-o", out, "-ldl"], env=tknn._env())
-    return out
+    return cpp_main.build("clusters_main", outdir)
 
 
 def run(exe, workdir, xyz, tolerance, min_size=1, max_size=2 ** 31 - 1, preload=None):
     """-> None when the call threw, else the clusters: a list of int32 index arrays, in the function's order"""
     xyz = np.ascontiguousarray(xyz, _f).reshape(-1, 3)
-    src, dst = os.path.join(str(workdir), "in.bin"), os.path.join(str(workdir), "out.bin")
-    with open(src, "wb") as f:
-        f.write(np.int32(len(xyz)).tobytes() + xyz.tobytes())
-    env = dict(os.environ)
-    if preload:
-        env["LD_PRELOAD"] = preload
-    r = subprocess.run([exe, src, dst, repr(float(tolerance)), str(int(min_size)), str(int(max_size))], env=env,
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, (r.returncode, r.stdout[-2000:], r.stderr[-2000:])
-    buf = np.frombuffer(open(dst, "rb").read(), np.int32)
+    buf = np.frombuffer(cpp_main.run(exe, workdir, np.int32(len(xyz)).tobytes() + xyz.tobytes(),
+                                     [repr(float(tolerance)), str(int(min_size)), str(int(max_size))], preload), np.int32)
     if buf[0]:
         return None
     out, at = [], 2

@@ -1,77 +1,34 @@
 """Builds and runs tests/cpp/correspondences_main.cc, the test program of Match4PCSBase::getCorrespondences, for
-tests/test_verify_nearest_cpu.py (on the oracle stand-in) and tests/test_verify_nearest_gpu.py (on the real library), and
-the stand-in's companion that answers s4g_verify_nearest on the CPU (tests/stubs/s4g_nearest_shim.cc)."""
-import os
-import subprocess
-
+tests/test_verify_nearest_cpu.py (on the oracle stand-in) and tests/test_verify_nearest_gpu.py (on the real library).
+Also the input of every test program that registers a pair of clouds first (this one, nearest_any, range, knn)."""
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from tests import cpp_main
 
 
 def build(outdir):
-    """compiles the program into `outdir` against the C++ layer; None when the layer or Eigen is missing"""
-    from oracle import _build
-    from super4pcs_b200 import build_cpp
-    if build_cpp.build_all()["lib"] is None:
-        return None
-    eig = None
-    for c in (os.environ.get("S4_EIGEN_ROOT"), os.path.join(_build.REFERENCE_ROOT, "3rdparty", "Eigen"), "/usr/include/eigen3"):
-        if c and os.path.exists(os.path.join(c, "Eigen", "Core")):
-            eig = c
-            break
-    if eig is None:
-        return None
-    libdir = os.path.join(ROOT, "super4pcs_b200", "lib")
-    exe = os.path.join(str(outdir), "correspondences_main")
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    env.pop("CC", None)
-    subprocess.check_call(["g++", "-std=c++14", "-O2", "-w", "-I", os.path.join(ROOT, "include"), "-I", eig,
-                           os.path.join(ROOT, "tests", "cpp", "correspondences_main.cc"), "-o", exe, "-L", libdir,
-                           "-lsuper4pcs_b200", "-ls4g", "-Wl,-rpath," + libdir], env=env)
-    return exe
+    return cpp_main.build("correspondences_main", outdir)
 
 
-def build_nearest_shim(outdir):
-    """compiles tests/stubs/s4g_nearest_shim.cc (+ the brute force of oracle/nearest_port.cc) into `outdir`; preload it
-    ahead of the oracle stand-in of libs4g"""
-    out = os.path.join(str(outdir), "libs4g_nearest_shim.so")
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    env.pop("CC", None)
-    subprocess.check_call(["g++", "-std=c++14", "-O2", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
-                           "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "stubs", "s4g_nearest_shim.cc"),
-                           os.path.join(ROOT, "oracle", "nearest_port.cc"), "-o", out, "-ldl"], env=env)
-    return out
+def run_pair(exe, workdir, P, Q, delta, overlap, sample_size, preload):
+    """runs a program that calls ComputeTransformation(P, Q) at (delta, overlap, sample_size) first -> a Reader of its
+    output"""
+    P, Q = np.ascontiguousarray(P, np.float32), np.ascontiguousarray(Q, np.float32)
+    payload = np.array([len(P), len(Q)], np.int32).tobytes() + P.tobytes() + Q.tobytes()
+    args = [repr(float(delta)), repr(float(overlap)), str(int(sample_size))]
+    return cpp_main.Reader(cpp_main.run(exe, workdir, payload, args, preload))
 
 
 def run(exe, workdir, P, Q, delta, overlap, sample_size, preload=None):
     """ComputeTransformation + getCorrespondences -> dict(threw_before, score, T, C (centred), sP, sQ, nearest, sq,
     nearest2 (the call without sq_dist))"""
-    P, Q = np.ascontiguousarray(P, np.float32), np.ascontiguousarray(Q, np.float32)
-    src, dst = os.path.join(str(workdir), "in.bin"), os.path.join(str(workdir), "out.bin")
-    with open(src, "wb") as f:
-        f.write(np.array([len(P), len(Q)], np.int32).tobytes() + P.tobytes() + Q.tobytes())
-    env = dict(os.environ)
-    if preload:
-        env["LD_PRELOAD"] = preload
-    r = subprocess.run([exe, src, dst, repr(float(delta)), repr(float(overlap)), str(int(sample_size))], env=env,
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, (r.returncode, r.stdout[-2000:], r.stderr[-2000:])
-    b = open(dst, "rb").read()
-    at = 0
-
-    def take(dt, n):
-        nonlocal at
-        a = np.frombuffer(b, dt, n, at).copy()
-        at += a.nbytes
-        return a
+    r = run_pair(exe, workdir, P, Q, delta, overlap, sample_size, preload)
+    take = r.take
     out = dict(threw_before=int(take(np.int32, 1)[0]), score=take(np.float32, 1)[0], T=take(np.float32, 16),
                C=take(np.float32, 16))
     out["sP"] = take(np.float32, 3 * int(take(np.int32, 1)[0])).reshape(-1, 3)
     out["sQ"] = take(np.float32, 3 * int(take(np.int32, 1)[0])).reshape(-1, 3)
     nq = len(out["sQ"])
     out["nearest"], out["sq"], out["nearest2"] = take(np.int32, nq), take(np.float32, nq), take(np.int32, nq)
-    assert at == len(b)
+    assert r.done()
     return out

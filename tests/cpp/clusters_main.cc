@@ -1,5 +1,5 @@
 // Test program of Utils::ExtractEuclideanClusters (tests/test_clusters_cpu.py, tests/test_clusters_gpu.py).  Linked
-// against the C++ layer; with LD_PRELOAD of the oracle stand-in (and tests/stubs/s4g_clusters_shim.cc) it runs on the CPU.
+// against the C++ layer; with LD_PRELOAD of the oracle stand-in it runs on the CPU.
 //   clusters_main IN OUT tolerance min_size max_size
 // IN : int32 n, float32 xyz[n][3]
 // OUT: int32 threw (1: the call threw; nothing else follows), int32 n_clusters, then per cluster int32 size and its

@@ -1,9 +1,9 @@
 // Test program of Utils::ComputeFPFH and Utils::MatchFPFH (tests/test_fpfh_cpu.py, tests/test_fpfh_gpu.py).  Linked
-// against the C++ layer; with LD_PRELOAD of the oracle stand-in (and tests/stubs/s4g_fpfh_shim.cc) it runs on the CPU.
-//   fpfh_main compute IN OUT k max_distance
+// against the C++ layer; with LD_PRELOAD of the oracle stand-in it runs on the CPU.
+//   fpfh_main IN OUT compute k max_distance
 //     IN : int32 n, float32 xyz[n][3], float32 normals[n][3] (stored through Point3D::set_normal)
 //     OUT: int32 threw (1: ComputeFPFH threw), float32 fpfh[n][33] (when it did not throw)
-//   fpfh_main match IN OUT mutual
+//   fpfh_main IN OUT match mutual
 //     IN : int32 n_source, int32 n_target, float32 source[n_source][33], float32 target[n_target][33]
 //     OUT: int32 threw (1: MatchFPFH threw), int32 index[n_source] (when it did not throw)
 #include "super4pcs/utils/features.h"
@@ -18,12 +18,12 @@ using namespace GlobalRegistration;
 
 int main(int argc, char** argv) {
   if (argc < 4) return 2;
-  FILE* in = std::fopen(argv[2], "rb");
+  FILE* in = std::fopen(argv[1], "rb");
   if (!in) return 2;
   int threw = 0;
   std::vector<float> outf;
   std::vector<int> outi;
-  if (std::strcmp(argv[1], "compute") == 0 && argc == 6) {
+  if (std::strcmp(argv[3], "compute") == 0 && argc == 6) {
     int n = 0;
     if (std::fread(&n, sizeof(int), 1, in) != 1) return 2;
     std::vector<float> raw(6 * size_t(n));
@@ -40,7 +40,7 @@ int main(int argc, char** argv) {
     } catch (const std::runtime_error&) {
       threw = 1;
     }
-  } else if (std::strcmp(argv[1], "match") == 0 && argc == 5) {
+  } else if (std::strcmp(argv[3], "match") == 0 && argc == 5) {
     int ns = 0, nt = 0;
     if (std::fread(&ns, sizeof(int), 1, in) != 1 || std::fread(&nt, sizeof(int), 1, in) != 1) return 2;
     std::vector<Utils::FPFHSignature> s(ns), t(nt);
@@ -57,7 +57,7 @@ int main(int argc, char** argv) {
     return 2;
   }
   std::fclose(in);
-  FILE* out = std::fopen(argv[3], "wb");
+  FILE* out = std::fopen(argv[2], "wb");
   if (!out) return 2;
   std::fwrite(&threw, sizeof(int), 1, out);
   if (!outf.empty()) std::fwrite(outf.data(), sizeof(float), outf.size(), out);

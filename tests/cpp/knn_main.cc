@@ -1,7 +1,6 @@
 // Test program of Match4PCSBase::getKNearest (tests/test_knn_cpu.py, tests/test_knn_gpu.py): runs
 // MatchSuper4PCS::ComputeTransformation on two clouds, then the k nearest neighbours under the found transform for a few
-// (k, max_distance).  Linked against the C++ layer; with LD_PRELOAD of the oracle stand-in (and
-// tests/stubs/s4g_knn_shim.cc) it runs on the CPU.
+// (k, max_distance).  Linked against the C++ layer; with LD_PRELOAD of the oracle stand-in it runs on the CPU.
 //   knn_main IN OUT delta overlap sample_size
 // IN : int32 nP, int32 nQ, float32 P[nP][3], float32 Q[nQ][3]
 // OUT: int32 threw_before (1: getKNearest threw before any registration), float32 score, float32 C[16] (the centred

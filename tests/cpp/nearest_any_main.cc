@@ -1,8 +1,7 @@
 // Test program of Match4PCSBase::MeanDistance and getCorrespondences(nearest, sq_dist, max_distance)
 // (tests/test_nearest_any_cpu.py, tests/test_nearest_any_gpu.py): runs MatchSuper4PCS::ComputeTransformation on two
 // clouds, then MeanDistance and the correspondences of the found transform at max_distance = delta, 3 delta and +inf.
-// Linked against the C++ layer; with LD_PRELOAD of the oracle stand-in (and tests/stubs/s4g_nearest_any_shim.cc) it
-// runs on the CPU.
+// Linked against the C++ layer; with LD_PRELOAD of the oracle stand-in it runs on the CPU.
 //   nearest_any_main IN OUT delta overlap sample_size
 // IN : int32 nP, int32 nQ, float32 P[nP][3], float32 Q[nQ][3]
 // OUT: int32 threw_before (1: the overload threw before any registration), float32 score, float32 T[16] (the returned

@@ -1,5 +1,5 @@
 // Test program of Utils::EstimateNormals (tests/test_normals_cpu.py, tests/test_normals_gpu.py).  Linked against the C++
-// layer; with LD_PRELOAD of the oracle stand-in (and tests/stubs/s4g_normals_shim.cc) it runs on the CPU.
+// layer; with LD_PRELOAD of the oracle stand-in it runs on the CPU.
 //   normals_main IN OUT k max_distance [vx vy vz]
 // IN : int32 n, float32 xyz[n][3]
 // OUT: int32 threw (1: EstimateNormals threw; nothing else follows), int32 returned count, float32 normals[n][3] (what

@@ -1,6 +1,5 @@
 // Test program of Utils::OrientNormals (tests/test_orient_normals_cpu.py, tests/test_orient_normals_gpu.py).  Linked
-// against the C++ layer; with LD_PRELOAD of the oracle stand-in (and tests/stubs/s4g_orient_normals_shim.cc) it runs on
-// the CPU.
+// against the C++ layer; with LD_PRELOAD of the oracle stand-in it runs on the CPU.
 //   orient_normals_main IN OUT k max_distance [vx vy vz]
 // IN : int32 n, float32 xyz[n][3], float32 normals[n][3] (stored through Point3D::set_normal)
 // OUT: int32 threw (1: OrientNormals threw), int32 returned count (0 when it threw), float32 normals[n][3] (what

@@ -1,6 +1,6 @@
 // Test program of Utils::RemoveStatisticalOutliers and Utils::RemoveRadiusOutliers (tests/test_outliers_cpu.py,
-// tests/test_outliers_gpu.py).  Linked against the C++ layer; with LD_PRELOAD of the oracle stand-in (and
-// tests/stubs/s4g_outliers_shim.cc) it runs on the CPU.
+// tests/test_outliers_gpu.py).  Linked against the C++ layer; with LD_PRELOAD of the oracle stand-in it runs on
+// the CPU.
 //   outliers_main IN OUT statistical k std_ratio
 //   outliers_main IN OUT radius radius min_neighbors
 // IN : int32 n, float32 xyz[n][3], float32 normals[n][3], float32 rgb[n][3]

@@ -1,5 +1,5 @@
 // Test program of Utils::SegmentPlanes (tests/test_planes_cpu.py, tests/test_planes_gpu.py).  Linked against the C++
-// layer; with LD_PRELOAD of the oracle stand-in (and tests/stubs/s4g_planes_shim.cc) it runs on the CPU.
+// layer; with LD_PRELOAD of the oracle stand-in it runs on the CPU.
 //   planes_main IN OUT threshold max_planes min_inliers iterations seed refine
 // IN : int32 n, float32 xyz[n][3]
 // OUT: int32 threw (1: the call threw; nothing else follows), int32 n_planes, then per plane float32 coefficients[4],

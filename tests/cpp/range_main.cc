@@ -1,7 +1,7 @@
 // Test program of Match4PCSBase::getNeighbors (tests/test_range_cpu.py, tests/test_range_gpu.py): runs
 // MatchSuper4PCS::ComputeTransformation on two clouds, then the neighbours of the found transform at max_distance =
-// delta and 3 delta.  Linked against the C++ layer; with LD_PRELOAD of the oracle stand-in (and
-// tests/stubs/s4g_range_shim.cc) it runs on the CPU.
+// delta and 3 delta.  Linked against the C++ layer; with LD_PRELOAD of the oracle stand-in it runs on the
+// CPU.
 //   range_main IN OUT delta overlap sample_size
 // IN : int32 nP, int32 nQ, float32 P[nP][3], float32 Q[nQ][3]
 // OUT: int32 threw_before (1: getNeighbors threw before any registration), float32 score, float32 C[16] (the centred

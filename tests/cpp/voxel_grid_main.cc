@@ -1,5 +1,5 @@
 // Test program of Utils::VoxelGridFilter (tests/test_voxel_grid_cpu.py, tests/test_voxel_grid_gpu.py).  Linked against
-// the C++ layer; with LD_PRELOAD of the oracle stand-in (and tests/stubs/s4g_voxel_grid_shim.cc) it runs on the CPU.
+// the C++ layer; with LD_PRELOAD of the oracle stand-in it runs on the CPU.
 //   voxel_grid_main IN OUT leaf min_points
 // IN : int32 n, int32 has_rgb, float32 xyz[n][3], float32 normals[n][3], float32 rgb[n][3] (used when has_rgb)
 // OUT: int32 threw (1: the call threw; the cloud as it is afterwards follows all the same), int32 returned count,

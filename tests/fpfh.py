@@ -1,17 +1,13 @@
 """Builds and runs tests/cpp/fpfh_main.cc, the test program of Utils::ComputeFPFH and Utils::MatchFPFH, for
-tests/test_fpfh_cpu.py (on the oracle stand-in) and tests/test_fpfh_gpu.py (on the real library), and the stand-in's
-companion that answers s4g_fpfh and s4g_fpfh_match on the CPU (tests/stubs/s4g_fpfh_shim.cc).  Also restatements that
+tests/test_fpfh_cpu.py (on the oracle stand-in) and tests/test_fpfh_gpu.py (on the real library).  Also restatements that
 share no code with the port: Open3D's formulas in numpy float64 (atan2, acos, hist_incr added per pair, S_h interleaved
 with the sums), the s4g_fpfh contract in plain Python doubles, and the match in numpy float32 column by column."""
 import math
-import os
-import subprocess
 
 import numpy as np
 
-from tests import knn as tknn
+from tests import cpp_main
 
-ROOT = tknn.ROOT
 _f = np.float32
 
 # c_i, s_i of beta_i = -pi + 2 pi i / 11, i = 1..5 (include/s4g.h), as the contract tabulates them
@@ -27,70 +23,28 @@ def face(i):
 
 
 def build(outdir):
-    """compiles the program into `outdir` against the C++ layer; None when the layer or Eigen is missing"""
-    from oracle import _build
-    from super4pcs_b200 import build_cpp
-    if build_cpp.build_all()["lib"] is None:
-        return None
-    eig = None
-    for c in (os.environ.get("S4_EIGEN_ROOT"), os.path.join(_build.REFERENCE_ROOT, "3rdparty", "Eigen"), "/usr/include/eigen3"):
-        if c and os.path.exists(os.path.join(c, "Eigen", "Core")):
-            eig = c
-            break
-    if eig is None:
-        return None
-    libdir = os.path.join(ROOT, "super4pcs_b200", "lib")
-    exe = os.path.join(str(outdir), "fpfh_main")
-    subprocess.check_call(["g++", "-std=c++14", "-O2", "-w", "-I", os.path.join(ROOT, "include"), "-I", eig,
-                           os.path.join(ROOT, "tests", "cpp", "fpfh_main.cc"), "-o", exe, "-L", libdir,
-                           "-lsuper4pcs_b200", "-ls4g", "-Wl,-rpath," + libdir], env=tknn._env())
-    return exe
-
-
-def build_shim(outdir):
-    """compiles tests/stubs/s4g_fpfh_shim.cc (+ oracle/fpfh_port.cc and oracle/knn_port.cc) into `outdir`; preload it
-    ahead of the oracle stand-in of libs4g"""
-    out = os.path.join(str(outdir), "libs4g_fpfh_shim.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O2", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
-                           "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "stubs", "s4g_fpfh_shim.cc"),
-                           os.path.join(ROOT, "oracle", "fpfh_port.cc"), os.path.join(ROOT, "oracle", "knn_port.cc"),
-                           "-o", out, "-ldl"], env=tknn._env())
-    return out
-
-
-def _run(args, preload):
-    env = dict(os.environ)
-    if preload:
-        env["LD_PRELOAD"] = preload
-    r = subprocess.run(args, env=env, capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, (r.returncode, r.stdout[-2000:], r.stderr[-2000:])
+    return cpp_main.build("fpfh_main", outdir)
 
 
 def run_compute(exe, workdir, xyz, normals, k, max_distance=np.inf, preload=None):
     """-> None when ComputeFPFH threw, else its descriptors [n, 33] float32"""
     xyz = np.ascontiguousarray(xyz, _f).reshape(-1, 3)
-    src, dst = os.path.join(str(workdir), "in.bin"), os.path.join(str(workdir), "out.bin")
-    with open(src, "wb") as f:
-        f.write(np.int32(len(xyz)).tobytes() + xyz.tobytes() + np.ascontiguousarray(normals, _f).tobytes())
-    _run([exe, "compute", src, dst, str(int(k)), repr(float(max_distance))], preload)
-    b = open(dst, "rb").read()
-    if np.frombuffer(b, np.int32, 1)[0]:
+    payload = np.int32(len(xyz)).tobytes() + xyz.tobytes() + np.ascontiguousarray(normals, _f).tobytes()
+    r = cpp_main.Reader(cpp_main.run(exe, workdir, payload, ["compute", str(int(k)), repr(float(max_distance))], preload))
+    if r.take(np.int32, 1)[0]:
         return None
-    return np.frombuffer(b, _f, 33 * len(xyz), 4).reshape(-1, 33).copy()
+    return r.take(_f, 33 * len(xyz)).reshape(-1, 33)
 
 
 def run_match(exe, workdir, source, target, mutual=True, preload=None):
     """-> None when MatchFPFH threw, else its indices [n_source] int32"""
     S = np.ascontiguousarray(source, _f).reshape(-1, 33)
     T = np.ascontiguousarray(target, _f).reshape(-1, 33)
-    src, dst = os.path.join(str(workdir), "in.bin"), os.path.join(str(workdir), "out.bin")
-    with open(src, "wb") as f:
-        f.write(np.int32(len(S)).tobytes() + np.int32(len(T)).tobytes() + S.tobytes() + T.tobytes())
-    _run([exe, "match", src, dst, str(int(bool(mutual)))], preload)
-    b = open(dst, "rb").read()
-    if np.frombuffer(b, np.int32, 1)[0]:
+    payload = np.int32(len(S)).tobytes() + np.int32(len(T)).tobytes() + S.tobytes() + T.tobytes()
+    r = cpp_main.Reader(cpp_main.run(exe, workdir, payload, ["match", str(int(bool(mutual)))], preload))
+    if r.take(np.int32, 1)[0]:
         return None
-    return np.frombuffer(b, np.int32, len(S), 4).copy()
+    return r.take(np.int32, len(S))
 
 
 # ---- surfaces

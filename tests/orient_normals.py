@@ -1,69 +1,28 @@
 """Builds and runs tests/cpp/orient_normals_main.cc, the test program of Utils::OrientNormals, for
-tests/test_orient_normals_cpu.py (on the oracle stand-in) and tests/test_orient_normals_gpu.py (on the real library), and
-the stand-in's companion that answers s4g_orient_normals on the CPU (tests/stubs/s4g_orient_normals_shim.cc).  Also two
-restatements of the s4g_orient_normals contract that share no code with the port (scipy's minimum spanning tree and a
+tests/test_orient_normals_cpu.py (on the oracle stand-in) and tests/test_orient_normals_gpu.py (on the real library).
+Also two restatements of the s4g_orient_normals contract that share no code with the port (scipy's minimum spanning tree and a
 plain-Python Kruskal), and the shapes with analytic normals the tests share."""
-import os
-import subprocess
-
 import numpy as np
 
-from tests import knn as tknn, normals as tnormals
+from tests import cpp_main, normals as tnormals
 
-ROOT = tknn.ROOT
 _f = np.float32
 
 
 def build(outdir):
-    """compiles the program into `outdir` against the C++ layer; None when the layer or Eigen is missing"""
-    from oracle import _build
-    from super4pcs_b200 import build_cpp
-    if build_cpp.build_all()["lib"] is None:
-        return None
-    eig = None
-    for c in (os.environ.get("S4_EIGEN_ROOT"), os.path.join(_build.REFERENCE_ROOT, "3rdparty", "Eigen"), "/usr/include/eigen3"):
-        if c and os.path.exists(os.path.join(c, "Eigen", "Core")):
-            eig = c
-            break
-    if eig is None:
-        return None
-    libdir = os.path.join(ROOT, "super4pcs_b200", "lib")
-    exe = os.path.join(str(outdir), "orient_normals_main")
-    subprocess.check_call(["g++", "-std=c++14", "-O2", "-w", "-I", os.path.join(ROOT, "include"), "-I", eig,
-                           os.path.join(ROOT, "tests", "cpp", "orient_normals_main.cc"), "-o", exe, "-L", libdir,
-                           "-lsuper4pcs_b200", "-ls4g", "-Wl,-rpath," + libdir], env=tknn._env())
-    return exe
-
-
-def build_shim(outdir):
-    """compiles tests/stubs/s4g_orient_normals_shim.cc (+ oracle/orient_normals_port.cc and oracle/knn_port.cc) into
-    `outdir`; preload it ahead of the oracle stand-in of libs4g"""
-    out = os.path.join(str(outdir), "libs4g_orient_normals_shim.so")
-    subprocess.check_call(["g++", "-std=c++14", "-O2", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
-                           "-I", os.path.join(ROOT, "include"),
-                           os.path.join(ROOT, "tests", "stubs", "s4g_orient_normals_shim.cc"),
-                           os.path.join(ROOT, "oracle", "orient_normals_port.cc"),
-                           os.path.join(ROOT, "oracle", "knn_port.cc"), "-o", out, "-ldl"], env=tknn._env())
-    return out
+    return cpp_main.build("orient_normals_main", outdir)
 
 
 def run(exe, workdir, xyz, normals, k, max_distance=np.inf, viewpoint=None, preload=None):
     """-> (threw, returned count, normals [n, 3] float32 as the points hold them afterwards)"""
     xyz = np.ascontiguousarray(xyz, _f).reshape(-1, 3)
-    src, dst = os.path.join(str(workdir), "in.bin"), os.path.join(str(workdir), "out.bin")
-    with open(src, "wb") as f:
-        f.write(np.int32(len(xyz)).tobytes() + xyz.tobytes() + np.ascontiguousarray(normals, _f).tobytes())
-    env = dict(os.environ)
-    if preload:
-        env["LD_PRELOAD"] = preload
-    args = [exe, src, dst, str(int(k)), repr(float(max_distance))]
+    args = [str(int(k)), repr(float(max_distance))]
     if viewpoint is not None:
         args += [repr(float(v)) for v in np.asarray(viewpoint, _f)]
-    r = subprocess.run(args, env=env, capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, (r.returncode, r.stdout[-2000:], r.stderr[-2000:])
-    b = open(dst, "rb").read()
-    threw, count = np.frombuffer(b, np.int32, 2)
-    return bool(threw), int(count), np.frombuffer(b, _f, 3 * len(xyz), 8).reshape(-1, 3).copy()
+    payload = np.int32(len(xyz)).tobytes() + xyz.tobytes() + np.ascontiguousarray(normals, _f).tobytes()
+    r = cpp_main.Reader(cpp_main.run(exe, workdir, payload, args, preload))
+    threw, count = r.take(np.int32, 2)
+    return bool(threw), int(count), r.take(_f, 3 * len(xyz)).reshape(-1, 3)
 
 
 def expected_held(normals, oriented):

@@ -4,17 +4,12 @@
   of synth's bumpy-sphere surface, standing on it), with noise along the normals and uniform outliers;
 * a numpy restatement of the draws, the hypothesis planes and every hypothesis count of one round (float32 operations in
   numpy are IEEE, one rounding each, no contraction), independent of the C++ port;
-* the build and run of tests/cpp/planes_main.cc, the test program of Utils::SegmentPlanes, and of its CPU stand-in's
-  companion (tests/stubs/s4g_planes_shim.cc)."""
-import os
-import subprocess
-
+* the build and run of tests/cpp/planes_main.cc, the test program of Utils::SegmentPlanes."""
 import numpy as np
 
 from super4pcs_b200 import synth
-from tests import knn as tknn
+from tests import cpp_main
 
-ROOT = tknn.ROOT
 _f = np.float32
 M64 = np.uint64(0xFFFFFFFFFFFFFFFF)
 
@@ -148,50 +143,16 @@ def angle_deg(n1, n2):
 # ---- the C++ test program -------------------------------------------------------------------------------------------
 
 def build(outdir):
-    """compiles the program into `outdir` against the C++ layer; None when the layer or Eigen is missing"""
-    from oracle import _build
-    from super4pcs_b200 import build_cpp
-    if build_cpp.build_all()["lib"] is None:
-        return None
-    eig = None
-    for c in (os.environ.get("S4_EIGEN_ROOT"), os.path.join(_build.REFERENCE_ROOT, "3rdparty", "Eigen"), "/usr/include/eigen3"):
-        if c and os.path.exists(os.path.join(c, "Eigen", "Core")):
-            eig = c
-            break
-    if eig is None:
-        return None
-    libdir = os.path.join(ROOT, "super4pcs_b200", "lib")
-    exe = os.path.join(str(outdir), "planes_main")
-    subprocess.check_call(["g++", "-std=c++14", "-O2", "-w", "-I", os.path.join(ROOT, "include"), "-I", eig,
-                           os.path.join(ROOT, "tests", "cpp", "planes_main.cc"), "-o", exe, "-L", libdir,
-                           "-lsuper4pcs_b200", "-ls4g", "-Wl,-rpath," + libdir], env=tknn._env())
-    return exe
-
-
-def build_shim(outdir):
-    """compiles tests/stubs/s4g_planes_shim.cc (+ oracle/planes_port.cc) into `outdir`; preload it ahead of the oracle
-    stand-in of libs4g"""
-    out = os.path.join(str(outdir), "libs4g_planes_shim.so")
-    subprocess.check_call(["g++", "-std=c++14", "-O2", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
-                           "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "stubs", "s4g_planes_shim.cc"),
-                           os.path.join(ROOT, "oracle", "planes_port.cc"), "-o", out, "-ldl"], env=tknn._env())
-    return out
+    return cpp_main.build("planes_main", outdir)
 
 
 def run(exe, workdir, xyz, threshold, max_planes=1, min_inliers=1, iterations=1000, seed=0, refine=True, preload=None):
     """-> None when the call threw, else the planes: a list of (coefficients [4] float32, inliers int32 array)"""
     xyz = np.ascontiguousarray(xyz, _f).reshape(-1, 3)
-    src, dst = os.path.join(str(workdir), "in.bin"), os.path.join(str(workdir), "out.bin")
-    with open(src, "wb") as f:
-        f.write(np.int32(len(xyz)).tobytes() + xyz.tobytes())
-    env = dict(os.environ)
-    if preload:
-        env["LD_PRELOAD"] = preload
-    r = subprocess.run([exe, src, dst, repr(float(threshold)), str(int(max_planes)), str(int(min_inliers)),
-                        str(int(iterations)), str(int(seed)), "1" if refine else "0"], env=env, capture_output=True,
-                       text=True, timeout=900)
-    assert r.returncode == 0, (r.returncode, r.stdout[-2000:], r.stderr[-2000:])
-    buf = np.frombuffer(open(dst, "rb").read(), np.int32)
+    args = [repr(float(threshold)), str(int(max_planes)), str(int(min_inliers)), str(int(iterations)), str(int(seed)),
+            "1" if refine else "0"]
+    b = cpp_main.run(exe, workdir, np.int32(len(xyz)).tobytes() + xyz.tobytes(), args, preload)
+    buf = np.frombuffer(b, np.int32)
     if buf[0]:
         return None
     out, at = [], 2

@@ -1,74 +1,19 @@
 """Builds and runs tests/cpp/range_main.cc, the test program of Match4PCSBase::getNeighbors, for tests/test_range_cpu.py
-(on the oracle stand-in) and tests/test_range_gpu.py (on the real library), and the stand-in's companion that answers
-s4g_range on the CPU (tests/stubs/s4g_range_shim.cc)."""
-import os
-import subprocess
-
+(on the oracle stand-in) and tests/test_range_gpu.py (on the real library)."""
 import numpy as np
 
-from tests import nearest_any
-
-ROOT = nearest_any.ROOT
+from tests import correspondences, cpp_main
 
 
 def build(outdir):
-    """compiles the program into `outdir` against the C++ layer; None when the layer or Eigen is missing"""
-    from oracle import _build
-    from super4pcs_b200 import build_cpp
-    if build_cpp.build_all()["lib"] is None:
-        return None
-    eig = None
-    for c in (os.environ.get("S4_EIGEN_ROOT"), os.path.join(_build.REFERENCE_ROOT, "3rdparty", "Eigen"), "/usr/include/eigen3"):
-        if c and os.path.exists(os.path.join(c, "Eigen", "Core")):
-            eig = c
-            break
-    if eig is None:
-        return None
-    libdir = os.path.join(ROOT, "super4pcs_b200", "lib")
-    exe = os.path.join(str(outdir), "range_main")
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    env.pop("CC", None)
-    subprocess.check_call(["g++", "-std=c++14", "-O2", "-w", "-I", os.path.join(ROOT, "include"), "-I", eig,
-                           os.path.join(ROOT, "tests", "cpp", "range_main.cc"), "-o", exe, "-L", libdir,
-                           "-lsuper4pcs_b200", "-ls4g", "-Wl,-rpath," + libdir], env=env)
-    return exe
-
-
-def build_shim(outdir):
-    """compiles tests/stubs/s4g_range_shim.cc (+ the brute force of oracle/range_port.cc) into `outdir`; preload it
-    ahead of the oracle stand-in of libs4g"""
-    out = os.path.join(str(outdir), "libs4g_range_shim.so")
-    env = dict(os.environ)
-    env.pop("CXX", None)
-    env.pop("CC", None)
-    subprocess.check_call(["g++", "-std=c++14", "-O2", "-ffp-contract=off", "-fopenmp", "-fPIC", "-shared",
-                           "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "stubs", "s4g_range_shim.cc"),
-                           os.path.join(ROOT, "oracle", "range_port.cc"), "-o", out, "-ldl"], env=env)
-    return out
+    return cpp_main.build("range_main", outdir)
 
 
 def run(exe, workdir, P, Q, delta, overlap, sample_size, preload=None):
     """ComputeTransformation + getNeighbors at max_distance = delta, 3 delta -> dict(threw_before, score, C (centred),
     sP, sQ, max_distance [K], lists [K] of (offsets, indices, sq))"""
-    P, Q = np.ascontiguousarray(P, np.float32), np.ascontiguousarray(Q, np.float32)
-    src, dst = os.path.join(str(workdir), "in.bin"), os.path.join(str(workdir), "out.bin")
-    with open(src, "wb") as f:
-        f.write(np.array([len(P), len(Q)], np.int32).tobytes() + P.tobytes() + Q.tobytes())
-    env = dict(os.environ)
-    if preload:
-        env["LD_PRELOAD"] = preload
-    r = subprocess.run([exe, src, dst, repr(float(delta)), repr(float(overlap)), str(int(sample_size))], env=env,
-                       capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, (r.returncode, r.stdout[-2000:], r.stderr[-2000:])
-    b = open(dst, "rb").read()
-    at = 0
-
-    def take(dt, n):
-        nonlocal at
-        a = np.frombuffer(b, dt, n, at).copy()
-        at += a.nbytes
-        return a
+    r = correspondences.run_pair(exe, workdir, P, Q, delta, overlap, sample_size, preload)
+    take = r.take
     out = dict(threw_before=int(take(np.int32, 1)[0]), score=take(np.float32, 1)[0], C=take(np.float32, 16))
     out["sP"] = take(np.float32, 3 * int(take(np.int32, 1)[0])).reshape(-1, 3)
     out["sQ"] = take(np.float32, 3 * int(take(np.int32, 1)[0])).reshape(-1, 3)
@@ -79,5 +24,5 @@ def run(exe, workdir, P, Q, delta, overlap, sample_size, preload=None):
     for _ in range(K):
         off = take(np.int64, nq + 1)
         out["lists"].append((off, take(np.int32, int(off[-1])), take(np.float32, int(off[-1]))))
-    assert at == len(b)
+    assert r.done()
     return out

@@ -6,8 +6,11 @@
 // loop, speculative multi-base execution, visitor protocol, global transform) can be exercised
 // by the `-m "not gpu"` tests in a container without a GPU: tests/test_host_logic_cpu.py runs a
 // subprocess with LD_PRELOAD=<this library>, so the s4g_* symbols of the C++ layer resolve here
-// instead of to the CUDA library.  The product itself has no CPU path: libs4g.so fails with
-// S4G_ERR_CUDA when there is no device (tests/test_abi.py::test_no_cpu_fallback).
+// instead of to the CUDA library.  The point-cloud utilities (nearest, k-nearest and range queries,
+// normals, outliers, clusters, planes, voxel grid, FPFH) are answered by their restatements
+// (oracle/<name>_port.cc), compiled into this library, for the tests of the C++ layer's Utils.
+// The product itself has no CPU path: libs4g.so fails with S4G_ERR_CUDA when there is no device
+// (tests/test_abi.py::test_no_cpu_fallback).
 #include <atomic>
 #include <cmath>
 #include <condition_variable>
@@ -39,6 +42,37 @@ void port_get_pairs(void* h, int32_t* out);
 long port_find_quads(void* h, float invariant1, float invariant2, float distance_threshold2, const float* base_xyz,
                      const int32_t* pairs1, long n1, const int32_t* pairs2, long n2);
 void port_get_quads(void* h, int32_t* out);
+
+// the restatements of the point-cloud utilities, oracle/<name>_port.cc
+void nearest_bruteforce(const float* P, long nP, const float* Q, long nQ, float delta, const float* T16k, long K,
+                        int32_t* out_index, float* out_sq, uint32_t* out_counts);
+void nearest_any_bruteforce(const float* P, long nP, const float* X, long n, const float* T, float sq_radius,
+                            const int32_t* exclude, int32_t* out_index, float* out_sq);
+void knn_bruteforce(const float* P, long nP, const float* X, long n, const float* T, int k, float sq_radius,
+                    const int32_t* exclude, int32_t* out_index, float* out_sq);
+void range_bruteforce_count(const float* P, long nP, const float* X, long n, const float* T, float sq_radius,
+                            int64_t* offsets);
+void range_bruteforce_fill(const float* P, long nP, const float* X, long n, const float* T, float sq_radius,
+                           const int64_t* offsets, int32_t* out_index, float* out_sq);
+void normals_port(const float* P, long nP, const int64_t* which, long n, int k, float sq_radius, const float* viewpoint,
+                  float* normals, float* eig, int32_t* rows_out);
+int orient_normals_port(const float* P, long n, const float* normals, int k, float sq_radius, const float* viewpoint,
+                        const int32_t* rows_in, float* normals_out, int32_t* root, int64_t* out2, int32_t* tree_edges);
+void statistical_port(const float* P, long nP, int k, double std_ratio, uint8_t* flags, double* mean_dist,
+                      double* out2);
+void radius_port(const float* P, long nP, float sq_radius, int min_neighbors, int64_t* raw, int32_t* counts,
+                 uint8_t* flags);
+void clusters_port(const float* P, long n, float sq_radius, int min_size, int max_size, int32_t* labels, int32_t* root,
+                   int64_t* n_clusters, int64_t* offsets, int32_t* members);
+void planes_port(const float* P, long n, float threshold, int H, uint64_t seed, int refine, int max_planes,
+                 int64_t min_inliers, int32_t* labels, void* planes, int* n_planes, int64_t* offsets, int32_t* members,
+                 uint32_t* hyp_counts);
+int voxel_grid_port(const float* xyz, const float* normals, const float* rgb, long n, float leaf, int min_points,
+                    float* xyz_out, float* normals_out, float* rgb_out, int32_t* counts, int32_t* first,
+                    int32_t* voxel_of, int64_t* n_out);
+int fpfh_port(const float* P, long n, const float* normals, int k, float sq_radius, const int32_t* rows_in,
+              const float* sq_in, float* fpfh, double* spfh_out);
+void fpfh_match_port(const float* a, long na, const float* b, long nb, int mutual, int32_t* index, float* sq_dist);
 }
 
 // stand-in for the communicator of csrc/comm.cu: the shard threads of one base meet here and leave with the global record
@@ -60,6 +94,9 @@ struct s4g_ctx {
   bool has_n = false, has_rgb = false;
   float delta = 0;
   std::vector<int32_t> pairs[2], quads;
+  bool has_range = false;  // the lists of the last s4g_range, for s4g_get_range
+  std::vector<int32_t> range_index;
+  std::vector<float> range_sq;
   std::string err;
 };
 
@@ -91,11 +128,25 @@ int fail(s4g_ctx* c, int code, const char* msg) {
 }
 
 int ready(s4g_ctx* c) {
-  if (c->P.empty() || c->Q.empty()) return fail(c, S4G_ERR_STATE, "shim: call s4g_set_cloud_p and s4g_set_cloud_q first");
+  if (c->P.empty() || c->Q.empty())
+    return fail(c, S4G_ERR_STATE, "shim: call s4g_set_cloud_p and s4g_set_cloud_q first");
   if (c->port == nullptr)
     c->port = port_create(c->P.data(), int(c->P.size() / 3), c->Q.data(), c->has_n ? c->Qn.data() : nullptr,
                           c->has_rgb ? c->Qrgb.data() : nullptr, int(c->Q.size() / 3), c->delta);
   return S4G_OK;
+}
+
+// the point-cloud utilities need only the P cloud
+int need_p(s4g_ctx* c) { return c->P.empty() ? fail(c, S4G_ERR_STATE, "shim: call s4g_set_cloud_p first") : S4G_OK; }
+
+long n_p(const s4g_ctx* c) { return long(c->P.size() / 3); }
+
+// the flagged j, ascending
+void compact(const std::vector<uint8_t>& flags, int32_t* keep, int64_t* n_kept) {
+  int64_t m = 0;
+  for (std::size_t j = 0; j < flags.size(); ++j)
+    if (flags[j]) keep[m++] = int32_t(j);
+  *n_kept = m;
 }
 
 void drop_port(s4g_ctx* c) {
@@ -423,6 +474,170 @@ int s4g_get_timings(s4g_ctx* c, double* out5) {  // no device, no device time: e
 
 int s4g_voxel_sample(s4g_ctx* c, const float*, int64_t, float, int32_t*, int64_t*) {
   return c ? fail(c, S4G_ERR_STATE, "shim: s4g_voxel_sample is not provided (inputs < 200K points stay on the host)") : S4G_ERR_ARG;
+}
+
+// ---- the point-cloud utilities, answered by their restatements
+
+int s4g_verify_nearest(s4g_ctx* c, const float* T, int K, int32_t* index, float* sq_dist, uint32_t* counts) {
+  if (!c) return S4G_ERR_ARG;
+  if (K < 0 || (K > 0 && (!T || !index))) return fail(c, S4G_ERR_ARG, "shim: s4g_verify_nearest: bad arguments");
+  if (c->P.empty() || c->Q.empty())
+    return fail(c, S4G_ERR_STATE, "shim: call s4g_set_cloud_p and s4g_set_cloud_q first");
+  if (K > 0)
+    nearest_bruteforce(c->P.data(), n_p(c), c->Q.data(), long(c->Q.size() / 3), c->delta, T, K, index, sq_dist, counts);
+  return S4G_OK;
+}
+
+int s4g_nearest(s4g_ctx* c, const float* xyz, int n, const float* T, float sq_radius, const int32_t* exclude,
+                int32_t* index, float* sq_dist) {
+  if (!c) return S4G_ERR_ARG;
+  if (n < 0 || (n > 0 && (!xyz || !index)) || std::isnan(sq_radius))
+    return fail(c, S4G_ERR_ARG, "shim: s4g_nearest: bad arguments");
+  if (int rc = need_p(c)) return rc;
+  if (n > 0) nearest_any_bruteforce(c->P.data(), n_p(c), xyz, n, T, sq_radius, exclude, index, sq_dist);
+  return S4G_OK;
+}
+
+int s4g_knn(s4g_ctx* c, const float* xyz, int n, const float* T, int k, float sq_radius, const int32_t* exclude,
+            int32_t* index, float* sq_dist) {
+  if (!c) return S4G_ERR_ARG;
+  if (n < 0 || (n > 0 && (!xyz || !index)) || k < 1 || k > 64 || std::isnan(sq_radius))
+    return fail(c, S4G_ERR_ARG, "shim: s4g_knn: bad arguments");
+  if (int rc = need_p(c)) return rc;
+  knn_bruteforce(c->P.data(), n_p(c), xyz, n, T, k, sq_radius, exclude, index, sq_dist);
+  return S4G_OK;
+}
+
+int s4g_range(s4g_ctx* c, const float* xyz, int n, const float* T, float sq_radius, int64_t* offsets, int64_t* total) {
+  if (!c) return S4G_ERR_ARG;
+  if (n < 0 || (n > 0 && !xyz) || !offsets || !total || std::isnan(sq_radius))
+    return fail(c, S4G_ERR_ARG, "shim: s4g_range: bad arguments");
+  if (int rc = need_p(c)) return rc;
+  range_bruteforce_count(c->P.data(), n_p(c), xyz, n, T, sq_radius, offsets);
+  c->range_index.resize(size_t(offsets[n]));
+  c->range_sq.resize(size_t(offsets[n]));
+  range_bruteforce_fill(c->P.data(), n_p(c), xyz, n, T, sq_radius, offsets, c->range_index.data(), c->range_sq.data());
+  c->has_range = true;
+  *total = offsets[n];
+  return S4G_OK;
+}
+
+int s4g_get_range(s4g_ctx* c, int32_t* indices, float* sq_dist) {
+  if (!c) return S4G_ERR_ARG;
+  if (!c->has_range) return fail(c, S4G_ERR_STATE, "shim: call s4g_range first");
+  if (c->range_index.empty()) return S4G_OK;
+  if (!indices) return fail(c, S4G_ERR_ARG, "shim: s4g_get_range: bad arguments");
+  std::memcpy(indices, c->range_index.data(), c->range_index.size() * sizeof(int32_t));
+  if (sq_dist) std::memcpy(sq_dist, c->range_sq.data(), c->range_sq.size() * sizeof(float));
+  return S4G_OK;
+}
+
+int s4g_normals(s4g_ctx* c, int k, float sq_radius, const float* viewpoint, float* normals, float* eigenvalues) {
+  if (!c) return S4G_ERR_ARG;
+  if (k < 3 || k > 64 || std::isnan(sq_radius) || sq_radius < 0.f || !normals)
+    return fail(c, S4G_ERR_ARG, "shim: s4g_normals: bad arguments");
+  if (int rc = need_p(c)) return rc;
+  normals_port(c->P.data(), n_p(c), nullptr, n_p(c), k, sq_radius, viewpoint, normals, eigenvalues, nullptr);
+  return S4G_OK;
+}
+
+int s4g_orient_normals(s4g_ctx* c, const float* normals, int k, float sq_radius, const float* viewpoint,
+                       float* normals_out, int32_t* root, int64_t* out2, int32_t* tree_edges) {
+  if (!c) return S4G_ERR_ARG;
+  if (int rc = need_p(c)) return rc;
+  if (orient_normals_port(c->P.data(), n_p(c), normals, k, sq_radius, viewpoint, nullptr, normals_out, root, out2,
+                          tree_edges) != 0)
+    return fail(c, S4G_ERR_ARG, "shim: s4g_orient_normals: bad arguments");
+  return S4G_OK;
+}
+
+int s4g_statistical_outliers(s4g_ctx* c, int k, double std_ratio, int32_t* keep, int64_t* n_kept, double* mean_dist,
+                             double* out2) {
+  if (!c) return S4G_ERR_ARG;
+  if (k < 1 || k > 64 || !std::isfinite(std_ratio) || !keep || !n_kept)
+    return fail(c, S4G_ERR_ARG, "shim: s4g_statistical_outliers: bad arguments");
+  if (int rc = need_p(c)) return rc;
+  const long n = n_p(c);
+  std::vector<uint8_t> flags(static_cast<size_t>(n), 0);
+  std::vector<double> mean(static_cast<size_t>(n));
+  double o2[2];
+  statistical_port(c->P.data(), n, k, std_ratio, flags.data(), mean.data(), o2);
+  compact(flags, keep, n_kept);
+  if (mean_dist) std::memcpy(mean_dist, mean.data(), mean.size() * sizeof(double));
+  if (out2) out2[0] = o2[0], out2[1] = o2[1];
+  return S4G_OK;
+}
+
+int s4g_radius_outliers(s4g_ctx* c, float sq_radius, int min_neighbors, int32_t* keep, int64_t* n_kept, int32_t* counts) {
+  if (!c) return S4G_ERR_ARG;
+  if (std::isnan(sq_radius) || min_neighbors < 1 || !keep || !n_kept)
+    return fail(c, S4G_ERR_ARG, "shim: s4g_radius_outliers: bad arguments");
+  if (int rc = need_p(c)) return rc;
+  const long n = n_p(c);
+  std::vector<uint8_t> flags(static_cast<size_t>(n), 0);
+  std::vector<int32_t> cnt(static_cast<size_t>(n));
+  radius_port(c->P.data(), n, sq_radius, min_neighbors, nullptr, cnt.data(), flags.data());
+  compact(flags, keep, n_kept);
+  if (counts) std::memcpy(counts, cnt.data(), cnt.size() * sizeof(int32_t));
+  return S4G_OK;
+}
+
+int s4g_euclidean_clusters(s4g_ctx* c, float sq_radius, int min_size, int max_size, int32_t* labels, int32_t* root,
+                           int64_t* n_clusters, int64_t* offsets, int32_t* members) {
+  if (!c) return S4G_ERR_ARG;
+  if (std::isnan(sq_radius) || min_size < 1 || max_size < min_size || !labels || !n_clusters)
+    return fail(c, S4G_ERR_ARG, "shim: s4g_euclidean_clusters: bad arguments");
+  if (int rc = need_p(c)) return rc;
+  const long n = n_p(c);
+  std::vector<int64_t> off(static_cast<size_t>(n) + 1);
+  std::vector<int32_t> mem(static_cast<size_t>(n));
+  clusters_port(c->P.data(), n, sq_radius, min_size, max_size, labels, root, n_clusters, off.data(), mem.data());
+  if (offsets) std::memcpy(offsets, off.data(), size_t(*n_clusters + 1) * sizeof(int64_t));
+  if (members) std::memcpy(members, mem.data(), size_t(off[size_t(*n_clusters)]) * sizeof(int32_t));
+  return S4G_OK;
+}
+
+int s4g_segment_planes(s4g_ctx* c, float threshold, int n_hypotheses, uint64_t seed, int refine, int max_planes,
+                       int64_t min_inliers, int32_t* labels, s4g_plane* planes, int* n_planes, int64_t* offsets,
+                       int32_t* members, uint32_t* hyp_counts) {
+  if (!c) return S4G_ERR_ARG;
+  if (std::isnan(threshold) || threshold < 0.f || n_hypotheses < 1 || n_hypotheses > (1 << 20) || max_planes < 1 ||
+      min_inliers < 1 || !labels || !planes || !n_planes)
+    return fail(c, S4G_ERR_ARG, "shim: s4g_segment_planes: bad arguments");
+  if (int rc = need_p(c)) return rc;
+  const long n = n_p(c);
+  std::vector<int64_t> off(static_cast<size_t>(max_planes) + 1);
+  std::vector<int32_t> mem(static_cast<size_t>(n));
+  planes_port(c->P.data(), n, threshold, n_hypotheses, seed, refine, max_planes, min_inliers, labels, planes, n_planes,
+              off.data(), mem.data(), hyp_counts);
+  if (offsets) std::memcpy(offsets, off.data(), size_t(*n_planes + 1) * sizeof(int64_t));
+  if (members) std::memcpy(members, mem.data(), size_t(off[size_t(*n_planes)]) * sizeof(int32_t));
+  return S4G_OK;
+}
+
+// needs no cloud: the points are arguments
+int s4g_voxel_grid(s4g_ctx* c, const float* xyz, const float* normals, const float* rgb, int64_t n, float leaf,
+                   int min_points, float* xyz_out, float* normals_out, float* rgb_out, int32_t* counts, int32_t* first,
+                   int32_t* voxel_of, int64_t* n_out) {
+  if (!c || !xyz || !xyz_out || !n_out) return S4G_ERR_ARG;
+  return voxel_grid_port(xyz, normals, rgb, long(n), leaf, min_points, xyz_out, normals_out, rgb_out, counts, first,
+                         voxel_of, n_out);
+}
+
+int s4g_fpfh(s4g_ctx* c, const float* normals, int k, float sq_radius, float* fpfh) {
+  if (!c) return S4G_ERR_ARG;
+  if (int rc = need_p(c)) return rc;
+  if (fpfh_port(c->P.data(), n_p(c), normals, k, sq_radius, nullptr, nullptr, fpfh, nullptr) != 0)
+    return fail(c, S4G_ERR_ARG, "shim: s4g_fpfh: bad arguments");
+  return S4G_OK;
+}
+
+// needs no cloud: the descriptors are arguments
+int s4g_fpfh_match(s4g_ctx* c, const float* a, int64_t n_a, const float* b, int64_t n_b, int mutual, int32_t* index,
+                   float* sq_dist) {
+  if (!c || n_a < 0 || n_b < 0 || (n_a > 0 && (!a || !index)) || (n_a > 0 && n_b > 0 && !b)) return S4G_ERR_ARG;
+  if (n_a > 0) fpfh_match_port(a, long(n_a), b, long(n_b), mutual, index, sq_dist);
+  return S4G_OK;
 }
 
 }  // extern "C"

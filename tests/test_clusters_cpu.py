@@ -134,7 +134,7 @@ def program(s4g_lib, tmp_path_factory):
     exe = tcl.build(d)
     if exe is None:
         pytest.skip("C++ layer not buildable here (no Eigen)")
-    return exe, " ".join([tcl.build_shim(d), build_shim.build()])
+    return exe, build_shim.build()
 
 
 @pytest.mark.parametrize("tol,lo,hi", [(0.05, 1, INT_MAX), (0.05, 4, 5), (0.0, 1, INT_MAX), (float("inf"), 1, INT_MAX),

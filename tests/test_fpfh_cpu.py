@@ -255,7 +255,7 @@ def program(s4g_lib, tmp_path_factory):
     exe = tf.build(d)
     if exe is None:
         pytest.skip("C++ layer not buildable here (no Eigen)")
-    return exe, " ".join([tf.build_shim(d), build_shim.build()])
+    return exe, build_shim.build()
 
 
 @pytest.mark.parametrize("max_distance", [np.inf, 0.15])

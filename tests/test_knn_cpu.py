@@ -160,7 +160,7 @@ def program(s4g_lib, tmp_path_factory):
     exe = tknn.build(d)
     if exe is None:
         pytest.skip("C++ layer not buildable here (no Eigen)")
-    return exe, " ".join([tknn.build_shim(d), build_shim.build()])
+    return exe, build_shim.build()
 
 
 def check_program(r):

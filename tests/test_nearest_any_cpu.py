@@ -14,7 +14,7 @@ import numpy as np
 import pytest
 
 from oracle import nearest_any as ona
-from tests import common, correspondences, nearest_any
+from tests import common, nearest_any
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 needs_ref = pytest.mark.skipif(not ona.ref_available(), reason="oracle/_ref (compiled reference) not present")
@@ -177,8 +177,7 @@ def program(s4g_lib, tmp_path_factory):
     exe = nearest_any.build(d)
     if exe is None:
         pytest.skip("C++ layer not buildable here (no Eigen)")
-    # s4g_nearest from this shim, s4g_verify_nearest (the two-argument getCorrespondences) from the one before it
-    return exe, " ".join([nearest_any.build_shim(d), correspondences.build_nearest_shim(d), build_shim.build()])
+    return exe, build_shim.build()
 
 
 def check_program(r, delta, P=None):

@@ -186,7 +186,7 @@ def program(s4g_lib, tmp_path_factory):
     exe = tnormals.build(d)
     if exe is None:
         pytest.skip("C++ layer not buildable here (no Eigen)")
-    return exe, " ".join([tnormals.build_shim(d), build_shim.build()])
+    return exe, build_shim.build()
 
 
 @pytest.mark.parametrize("kind", ["synthetic", "plane_viewpoint", "radius", "duplicates"])

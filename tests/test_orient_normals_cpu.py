@@ -244,7 +244,7 @@ def program(s4g_lib, tmp_path_factory):
     exe = ton.build(d)
     if exe is None:
         pytest.skip("C++ layer not buildable here (no Eigen)")
-    return exe, " ".join([ton.build_shim(d), build_shim.build()])
+    return exe, build_shim.build()
 
 
 @pytest.mark.parametrize("vp", [None, (0.0, 0.0, 5.0)])

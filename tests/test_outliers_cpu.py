@@ -137,7 +137,7 @@ def program(s4g_lib, tmp_path_factory):
     exe = tout.build(d)
     if exe is None:
         pytest.skip("C++ layer not buildable here (no Eigen)")
-    return exe, " ".join([tout.build_shim(d), build_shim.build()])
+    return exe, build_shim.build()
 
 
 def attributes(n, seed):

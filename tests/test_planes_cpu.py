@@ -183,7 +183,7 @@ def program(s4g_lib, tmp_path_factory):
     exe = tp.build(d)
     if exe is None:
         pytest.skip("C++ layer not buildable here (no Eigen)")
-    return exe, " ".join([tp.build_shim(d), build_shim.build()])
+    return exe, build_shim.build()
 
 
 @pytest.mark.parametrize("thr,R,lo,H,seed,refine", [(0.01, 3, 100, 200, 0, True), (0.02, 1, 1, 50, 9, False),

@@ -114,7 +114,7 @@ def program(s4g_lib, tmp_path_factory):
     exe = trange.build(d)
     if exe is None:
         pytest.skip("C++ layer not buildable here (no Eigen)")
-    return exe, " ".join([trange.build_shim(d), build_shim.build()])
+    return exe, build_shim.build()
 
 
 def check_program(r):

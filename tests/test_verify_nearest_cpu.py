@@ -103,7 +103,7 @@ def program(s4g_lib, tmp_path_factory):
     exe = correspondences.build(d)
     if exe is None:
         pytest.skip("C++ layer not buildable here (no Eigen)")
-    return exe, correspondences.build_nearest_shim(d) + " " + build_shim.build()
+    return exe, build_shim.build()
 
 
 def test_get_correspondences_on_oracle_shim_hippo(program, tmp_path):

@@ -169,7 +169,7 @@ def program(s4g_lib, tmp_path_factory):
     exe = tvg.build(d)
     if exe is None:
         pytest.skip("C++ layer not buildable here (no Eigen)")
-    return exe, " ".join([tvg.build_shim(d), build_shim.build()])
+    return exe, build_shim.build()
 
 
 @pytest.mark.parametrize("colour", [True, False, "partial"])

@@ -1,47 +1,15 @@
 """Builds and runs tests/cpp/voxel_grid_main.cc, the test program of Utils::VoxelGridFilter, for
-tests/test_voxel_grid_cpu.py (on the oracle stand-in) and tests/test_voxel_grid_gpu.py (on the real library), and the
-stand-in's companion that answers s4g_voxel_grid on the CPU (tests/stubs/s4g_voxel_grid_shim.cc).  Also an independent
-numpy restatement of the s4g_voxel_grid contract, and the clouds the tests share."""
-import os
-import subprocess
-
+tests/test_voxel_grid_cpu.py (on the oracle stand-in) and tests/test_voxel_grid_gpu.py (on the real library).  Also an
+independent numpy restatement of the s4g_voxel_grid contract, and the clouds the tests share."""
 import numpy as np
 
-from tests import knn as tknn, normals as tnormals
+from tests import cpp_main, normals as tnormals
 
-ROOT = tknn.ROOT
 _f = np.float32
 
 
 def build(outdir):
-    """compiles the program into `outdir` against the C++ layer; None when the layer or Eigen is missing"""
-    from oracle import _build
-    from super4pcs_b200 import build_cpp
-    if build_cpp.build_all()["lib"] is None:
-        return None
-    eig = None
-    for c in (os.environ.get("S4_EIGEN_ROOT"), os.path.join(_build.REFERENCE_ROOT, "3rdparty", "Eigen"), "/usr/include/eigen3"):
-        if c and os.path.exists(os.path.join(c, "Eigen", "Core")):
-            eig = c
-            break
-    if eig is None:
-        return None
-    libdir = os.path.join(ROOT, "super4pcs_b200", "lib")
-    exe = os.path.join(str(outdir), "voxel_grid_main")
-    subprocess.check_call(["g++", "-std=c++14", "-O2", "-w", "-I", os.path.join(ROOT, "include"), "-I", eig,
-                           os.path.join(ROOT, "tests", "cpp", "voxel_grid_main.cc"), "-o", exe, "-L", libdir,
-                           "-lsuper4pcs_b200", "-ls4g", "-Wl,-rpath," + libdir], env=tknn._env())
-    return exe
-
-
-def build_shim(outdir):
-    """compiles tests/stubs/s4g_voxel_grid_shim.cc (+ oracle/voxel_grid_port.cc) into `outdir`; preload it ahead of
-    the oracle stand-in of libs4g"""
-    out = os.path.join(str(outdir), "libs4g_voxel_grid_shim.so")
-    subprocess.check_call(["g++", "-std=c++14", "-O2", "-ffp-contract=off", "-fPIC", "-shared",
-                           "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "stubs", "s4g_voxel_grid_shim.cc"),
-                           os.path.join(ROOT, "oracle", "voxel_grid_port.cc"), "-o", out], env=tknn._env())
-    return out
+    return cpp_main.build("voxel_grid_main", outdir)
 
 
 def run(exe, workdir, xyz, normals, rgb, leaf, min_points, preload=None):
@@ -51,18 +19,10 @@ def run(exe, workdir, xyz, normals, rgb, leaf, min_points, preload=None):
     has_rgb = rgb is not None
     rgb = np.zeros_like(xyz) if rgb is None else rgb
     blob = np.concatenate([xyz, np.asarray(normals, _f).reshape(-1, 3), np.asarray(rgb, _f).reshape(-1, 3)])
-    src, dst = os.path.join(str(workdir), "in.bin"), os.path.join(str(workdir), "out.bin")
-    with open(src, "wb") as f:
-        f.write(np.int32([len(xyz), int(has_rgb)]).tobytes() + np.ascontiguousarray(blob, _f).tobytes())
-    env = dict(os.environ)
-    if preload:
-        env["LD_PRELOAD"] = preload
-    r = subprocess.run([exe, src, dst, repr(float(leaf)), str(int(min_points))], env=env, capture_output=True, text=True,
-                       timeout=900)
-    assert r.returncode == 0, (r.returncode, r.stdout[-2000:], r.stderr[-2000:])
-    buf = open(dst, "rb").read()
-    threw, count, m = np.frombuffer(buf, np.int32, 3)
-    return bool(threw), int(count), np.frombuffer(buf, _f, 9 * int(m), 12).reshape(-1, 9).copy()
+    payload = np.int32([len(xyz), int(has_rgb)]).tobytes() + np.ascontiguousarray(blob, _f).tobytes()
+    r = cpp_main.Reader(cpp_main.run(exe, workdir, payload, [repr(float(leaf)), str(int(min_points))], preload))
+    threw, count, m = r.take(np.int32, 3)
+    return bool(threw), int(count), r.take(_f, 9 * int(m)).reshape(-1, 9)
 
 
 def held(xyz, normals, rgb):
