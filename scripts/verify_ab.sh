@@ -5,13 +5,13 @@
 #   bash scripts/verify_ab.sh
 #   VARIANTS='-DS4G_PROBE4|-DS4G_VERIFY_MIN_BLOCKS=10' bash scripts/verify_ab.sh        ('|' separates variants)
 # Knobs (super4pcs_b200/csrc/verify.cu): S4G_PROBE4 (four P points in flight per probe iteration instead of two),
-# S4G_VERIFY_MIN_BLOCKS (launch bound: resident CTAs per SM the register allocation aims at, default 12),
+# S4G_VERIFY_MIN_BLOCKS (launch bound: resident CTAs per SM the register allocation aims at, default 16),
 # S4G_QUEUE_CAP (shared-memory queue entries per round, default 3072).
 cd "$(dirname "$0")/.."
 mkdir -p ab_out
 OUT=${OUT:-ab_out/verify_ab.jsonl}
 : > "$OUT"
-IFS='|' read -r -a LIST <<< "${VARIANTS:-|-DS4G_PROBE4|-DS4G_VERIFY_MIN_BLOCKS=8|-DS4G_VERIFY_MIN_BLOCKS=10|-DS4G_VERIFY_MIN_BLOCKS=16|-DS4G_QUEUE_CAP=2048|-DS4G_QUEUE_CAP=4096|-DS4G_PROBE4 -DS4G_VERIFY_MIN_BLOCKS=10}"
+IFS='|' read -r -a LIST <<< "${VARIANTS:-|-DS4G_PROBE4|-DS4G_VERIFY_MIN_BLOCKS=8|-DS4G_VERIFY_MIN_BLOCKS=10|-DS4G_VERIFY_MIN_BLOCKS=12|-DS4G_QUEUE_CAP=2048|-DS4G_QUEUE_CAP=4096|-DS4G_PROBE4 -DS4G_VERIFY_MIN_BLOCKS=10}"
 for v in "${LIST[@]}"; do
   echo "== variant: '${v:-default}'"
   if ! S4G_NVCC_DEFINES="$v" timeout 300 python -c "from super4pcs_b200 import build; build.build_lib()" > ab_out/ab_build.log 2>&1; then

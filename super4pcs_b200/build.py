@@ -46,25 +46,29 @@ def _stale(target, deps):
     return any(os.path.getmtime(d) > t for d in deps if os.path.exists(d))
 
 
-def build_lib(force=False, verbose=False, extra_flags=()):
+def build_lib(force=False, verbose=False, extra_flags=(), out_dir=None):
+    """out_dir: build the objects and the library there instead of in the tree (variant builds that must not replace the
+    tree's library, scripts/verify_phases.py); returns the library's path"""
     nvcc = _nvcc()
-    os.makedirs(OBJ, exist_ok=True)
+    obj_dir = OBJ if out_dir is None else os.path.join(out_dir, "obj")
+    lib = LIB if out_dir is None else os.path.join(out_dir, "libs4g.so")
+    os.makedirs(obj_dir, exist_ok=True)
     headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
     headers.append(os.path.join(ROOT, "include", "s4g.h"))
     srcs = [s for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]
-    stamp, defines = os.path.join(OBJ, "defines.txt"), " ".join(_defines())
+    stamp, defines = os.path.join(obj_dir, "defines.txt"), " ".join(_defines())
     if (open(stamp).read() if os.path.exists(stamp) else "") != defines:
         force = True
     extra_flags = tuple(extra_flags) + tuple(_defines())
-    if not force and not _stale(LIB, [os.path.join(CSRC, s) for s in srcs] + headers):
-        return LIB                            # prebuilt library is current (e.g. on the GPU box)
+    if not force and not _stale(lib, [os.path.join(CSRC, s) for s in srcs] + headers):
+        return lib                            # prebuilt library is current (e.g. on the GPU box)
     env = dict(os.environ)
     env.pop("CXX", None)
     env.pop("CC", None)
     jobs = []
     for s in srcs:
         src = os.path.join(CSRC, s)
-        obj = os.path.join(OBJ, s.replace(".cu", ".o"))
+        obj = os.path.join(obj_dir, s.replace(".cu", ".o"))
         if force or _stale(obj, [src] + headers):
             jobs.append([nvcc, *NVCC_FLAGS, *extra_flags, "-c", src, "-o", obj])
 
@@ -78,9 +82,9 @@ def build_lib(force=False, verbose=False, extra_flags=()):
 
     with cf.ThreadPoolExecutor(max_workers=max(1, min(len(jobs), os.cpu_count() or 1))) as ex:
         outs = list(ex.map(run, jobs))
-    objs = [os.path.join(OBJ, s.replace(".cu", ".o")) for s in srcs]
-    if jobs or force or _stale(LIB, objs):
-        run([nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a",
+    objs = [os.path.join(obj_dir, s.replace(".cu", ".o")) for s in srcs]
+    if jobs or force or _stale(lib, objs):
+        run([nvcc, "-shared", "-o", lib, *objs, "-gencode", "arch=compute_90a,code=sm_90a",
              "-Xcompiler", "-fPIC", "-cudart", "static"])
     with open(stamp, "w") as f:
         f.write(defines)
@@ -88,7 +92,7 @@ def build_lib(force=False, verbose=False, extra_flags=()):
         for o in outs:
             if o:
                 print(o, file=sys.stderr)
-    return LIB
+    return lib
 
 
 if __name__ == "__main__":

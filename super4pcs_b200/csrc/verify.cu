@@ -63,13 +63,16 @@ constexpr int kTilesPerBlock = kThreads / 16;  // (tile, candidate) pairs of a C
 #define S4G_QUEUE_CAP 2048
 #endif
 #ifndef S4G_VERIFY_MIN_BLOCKS
-#define S4G_VERIFY_MIN_BLOCKS 12
+#define S4G_VERIFY_MIN_BLOCKS 16           // 16 CTAs (64 warps) per SM: 32 registers (DESIGN.md section 9)
 #endif
 #ifndef S4G_SUBVOXEL
 #define S4G_SUBVOXEL 1             // 0: ignore the second level of the delta-field (A/B)
 #endif
 #ifndef S4G_FLUSH_MIN
 #define S4G_FLUSH_MIN (S4G_QUEUE_CAP / 2)
+#endif
+#ifndef S4G_VERIFY_CLOCKS
+#define S4G_VERIFY_CLOCKS 0        // 1: k_verify<false, .> sums its SM cycles per phase (scripts/verify_phases.py)
 #endif
 constexpr int kQueueCap = S4G_QUEUE_CAP;   // queued pairs of a CTA (uint16 entries: candidate << 10 | tile << 7 | thread)
 constexpr int kWarpQueue = kQueueCap / (kThreads / 32);   // ... of one warp
@@ -80,6 +83,13 @@ static_assert(kTilesPerBlock == 8 && kCandPerBlock == 16, "entry layout: 4 + 3 +
 struct ProbeStats {
   unsigned long long tested = 0, ranges = 0, bricks = 0, bitmap = 0, culled = 0;
 };
+
+#if S4G_VERIFY_CLOCKS
+// SM cycles summed over the warps of every k_verify<false, .> launch: [0] staging and both cull levels, [1] the
+// delta-field look-ups of the tiles (the query load and the refinement included), [2] the queue and the exact test,
+// [3] everything (the rest of the tile loop and the final reduction are [3] - [0] - [1] - [2]).
+__device__ unsigned long long g_verify_clocks[4];
+#endif
 
 // Scan one contiguous run of P points; single exit, flag based.  Two points are in flight per
 // iteration (the loads of a run are independent; the kernel is latency-bound here).
@@ -267,6 +277,9 @@ k_verify(GridDev g, const float4* __restrict__ Q, const float4* __restrict__ til
   // candidate count known only on the device (s4g_try_bases): Kall is its upper bound
   const int K = dK != nullptr ? min(Kall, (int)__ldg(dK)) : Kall;
   if (qbase >= nQ || c0 >= K) return;             // CTA-uniform (the last patch may be short)
+  constexpr bool kClk = S4G_VERIFY_CLOCKS && !kStats;
+  uint32_t clk[4] = {0u, 0u, 0u, 0u};             // this warp's cycles per phase (g_verify_clocks; a CTA lasts << 2^32 cycles)
+  const uint32_t clk0 = kClk ? (uint32_t)clock() : 0u;
   const uint32_t* __restrict__ pp = perm != nullptr ? perm + (size_t)patch * Kall : nullptr;
   __shared__ __align__(16) float sT[kCandPerBlock * 12];     // exact transforms (decision arithmetic)
   __shared__ __align__(16) float sV[kCandPerBlock * 12];     // voxel-space transforms (selection only)
@@ -336,6 +349,7 @@ k_verify(GridDev g, const float4* __restrict__ Q, const float4* __restrict__ til
   int last_tile = 0;                              // last tile of this CTA that exists (CTA-uniform)
   for (int t = kTilesPerBlock - 1; t > 0; --t)
     if (qbase + (long long)t * kThreads < nQ) { last_tile = t; break; }
+  if (kClk) clk[0] = (uint32_t)clock() - clk0;
   unsigned long long cert = 0ull;                 // 4-bit counters: CERTAIN inliers of this thread's queries per candidate
 #pragma unroll 1
   for (int t = 0; t <= last_tile; ++t) {
@@ -344,6 +358,7 @@ k_verify(GridDev g, const float4* __restrict__ Q, const float4* __restrict__ til
     if (kStats) st.culled += (lane == 0 && tile0 + (tid & ~31) < nQ) ? (unsigned long long)(nc - __popc(live_mask)) : 0ull;
     const bool last = t == last_tile;
     if (live_mask == 0u && !last) continue;       // warp-uniform: nothing to do for this warp's 32 queries (no CTA barrier below)
+    uint32_t clk_t = kClk ? (uint32_t)clock() : 0u;
     const long long qi = tile0 + tid;
     const bool valid = qi < nQ;
     float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -414,6 +429,11 @@ k_verify(GridDev g, const float4* __restrict__ Q, const float4* __restrict__ til
         }
       }
     }
+    if (kClk) {
+      const uint32_t now = (uint32_t)clock();
+      clk[1] += now - clk_t;
+      clk_t = now;
+    }
     // ---- per-WARP queue: rounds of { compaction of pending pairs -> this warp's queue ; flush = phase 2 when enough
     // pairs wait, the queue is full, or this is the last tile }.  Warp-synchronous: no CTA barrier in the tile loop, the
     // four warps of the CTA drift apart freely (their live candidates differ).
@@ -465,6 +485,7 @@ k_verify(GridDev g, const float4* __restrict__ Q, const float4* __restrict__ til
         qn = 0u;
       }
     } while (again);
+    if (kClk) clk[2] += (uint32_t)clock() - clk_t;
   }
   // CERTAIN inliers: 16 packed 4-bit counters per thread -> one warp reduction per candidate
 #pragma unroll
@@ -484,6 +505,13 @@ k_verify(GridDev g, const float4* __restrict__ Q, const float4* __restrict__ til
     atomicAdd(&stats[3], st.bitmap);
     atomicAdd(&stats[4], st.culled);   // (32-query sub-tile, candidate) pairs culled (lane 0 of every warp counted them)
   }
+#if S4G_VERIFY_CLOCKS
+  if (kClk && lane == 0) {
+    clk[3] = (uint32_t)clock() - clk0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) atomicAdd(&g_verify_clocks[i], (unsigned long long)clk[i]);
+  }
+#endif
 }
 
 // ---- nearest P point within delta of every query (s4g_verify_nearest).  Same decision arithmetic as the exact test of
@@ -769,6 +797,24 @@ extern "C" int s4g_verify_probe_stats(s4g_ctx* ctx, const float* T, int K, uint6
   for (int i = 0; i < 5; ++i) out5[i] = h[i];
   return S4G_OK;
 }
+
+#if S4G_VERIFY_CLOCKS
+// Only in builds with -DS4G_VERIFY_CLOCKS=1 (not part of include/s4g.h): the phase cycles of g_verify_clocks summed since the
+// last reset, after the context's stream has finished; reset != 0 zeroes them afterwards.
+extern "C" int s4g_verify_clocks(s4g_ctx* ctx, uint64_t* out4, int reset) {
+  if (!ctx || !out4) return S4G_ERR_ARG;
+  S4G_CUDA(cudaSetDevice(ctx->device));
+  S4G_CUDA(cudaStreamSynchronize(ctx->stream));
+  unsigned long long h[4];
+  S4G_CUDA(cudaMemcpyFromSymbol(h, g_verify_clocks, sizeof(h)));
+  for (int i = 0; i < 4; ++i) out4[i] = h[i];
+  if (reset) {
+    const unsigned long long z[4] = {0, 0, 0, 0};
+    S4G_CUDA(cudaMemcpyToSymbol(g_verify_clocks, z, sizeof(z)));
+  }
+  return S4G_OK;
+}
+#endif
 
 extern "C" int s4g_verify_nearest_dev(s4g_ctx* ctx, const float* d_T, int K, int32_t* d_index, float* d_sq_dist,
                                       uint32_t* d_counts) {
