@@ -18,6 +18,8 @@
  *  - "host" pointers are ordinary CPU memory; functions with the suffix _dev take device
  *    pointers on the context's device and enqueue on the context's stream without
  *    synchronising (the caller owns ordering; see s4g_set_stream / s4g_synchronize).
+ *    The one exception is s4g_try_congruent_set_dev: it returns its record in host memory
+ *    (and reads the gate count back to size Verify), so it waits for the context's stream.
  *  - clouds are the CENTRED sampled clouds, i.e. what Match4PCSBase::init leaves in
  *    sampled_P_3D_ / sampled_Q_3D_ (algorithms/match4pcsBase.hpp:112-149).
  *  - there is no CPU fallback anywhere behind this ABI: without a CUDA device s4g_create fails.

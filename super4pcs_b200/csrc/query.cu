@@ -410,16 +410,26 @@ k_cluster_link(GridDev g, int n, float sq_radius, int* __restrict__ parent) {
   }
 }
 
-// the segments of one sort chunk (s4g_range): query i's list is [offsets[i], offsets[i + 1]); the chunk takes the lists
-// that start in [base, base + window), relative to base, and gives every other query an empty segment
-__global__ void k_range_chunk(const int64_t* __restrict__ offsets, int n, int64_t base, int64_t window,
-                              int* __restrict__ begin, int* __restrict__ end) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const int64_t b = offsets[i], e = offsets[i + 1];
-  const bool in = b >= base && b < base + window;
-  begin[i] = in ? (int)(b - base) : 0;
-  end[i] = in ? (int)(e - base) : 0;
+// the sort keys of one sort chunk (s4g_range): entry base + t of the output, in query i's list [offsets[i], offsets[i + 1]),
+// gets the key (i << jbits) | j, so that one radix sort of the chunk orders every list by j and keeps the lists in place
+__global__ void k_range_keys(const int64_t* __restrict__ offsets, int n, int64_t base, int len,
+                             const int32_t* __restrict__ indices, int jbits, unsigned long long* __restrict__ keys) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= len) return;
+  const int64_t p = base + t;
+  int lo = 0, hi = n - 1;   // the last i with offsets[i] <= p (offsets[0] = 0): the non-empty list that holds p
+  while (lo < hi) {
+    const int mid = lo + (hi - lo + 1) / 2;
+    if (offsets[mid] <= p) lo = mid; else hi = mid - 1;
+  }
+  keys[t] = ((unsigned long long)lo << jbits) | (unsigned)indices[p];
+}
+
+// the sorted keys of a chunk back to the indices they hold
+__global__ void k_range_unkey(const unsigned long long* __restrict__ keys, int len, unsigned long long jmask,
+                              int32_t* __restrict__ indices) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t < len) indices[t] = (int32_t)(keys[t] & jmask);
 }
 
 // ---- the k nearest P points within a radius, for arbitrary query points (s4g_knn).  One thread per query: y = T x
@@ -664,11 +674,14 @@ int range_count(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T, float
 }
 
 // enqueue the fill pass of k_range into d_indices / d_sq_dist (nullptr: not written) from d_offsets (total = its last
-// entry), then sort every list by index, its d^2 carried along.  CUB's segmented sort addresses the items with int, so the
-// lists are sorted in chunks: chunk c takes the lists that start in the window [c w, (c + 1) w) of the output, and a list
-// that starts there ends before c w + w + |P| <= c w + INT_MAX.  One chunk when total <= INT_MAX.  The sort ping-pongs
-// with a buffer of the chunk's size; when there is more than one chunk, that buffer starts as a copy of the output, so
-// the entries of the neighbouring chunks are copied back unchanged.
+// entry), then sort every list by index, its d^2 carried along: one radix sort of the keys (list, index), which leaves
+// every list where it is.  (Not CUB's segmented sort: with more than a few hundred segments it reads its partition sizes
+// back to the host and synchronises the stream.)  The sort addresses the items with int, so the lists are sorted in
+// chunks: chunk c sorts the w + |P| entries of the output from c w on (at most INT_MAX), which hold every list that starts
+// in the window [c w, (c + 1) w), since a list has at most |P| entries.  A list cut off at the chunk's start is the
+// suffix of a list an earlier chunk sorted whole, so it stays sorted; one cut off at its end starts in a later window,
+// whose chunk sorts it whole.  One chunk when total <= INT_MAX.  The scratch is 20 bytes per entry of a chunk: the keys
+// and their double buffer, and the double buffer of the d^2.
 int range_fill(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T, float sq_radius, const int64_t* d_offsets,
                int64_t total, int32_t* d_indices, float* d_sq_dist) {
   S4G_CUDA(cudaSetDevice(ctx->device));
@@ -681,38 +694,34 @@ int range_fill(s4g_ctx* ctx, const float* d_xyz, int n, const float* d_T, float 
   const int64_t kMaxItems = 0x7fffffff;
   int64_t window = total <= kMaxItems ? total : std::max<int64_t>(1, kMaxItems - ctx->nP);
   if (ctx->range_window > 0) window = std::min<int64_t>(window, ctx->range_window);
-  const bool chunked = window < total;
-  S4G_TRY(s4g_reserve(ctx, ctx->dScratchD, 2 * (size_t)n * sizeof(int)));
-  int* seg_begin = ctx->dScratchD.as<int>();
-  int* seg_end = seg_begin + n;
+  auto bits = [](unsigned v) { return v ? 32 - __builtin_clz(v) : 0; };
+  const int jbits = bits((unsigned)(ctx->nP - 1)), end_bit = std::max(1, jbits + bits((unsigned)(n - 1)));
+  const unsigned long long jmask = (1ull << jbits) - 1;
   for (int64_t base = 0; base < total; base += window) {
-    const int len = (int)std::min<int64_t>(total - base, kMaxItems);
-    S4G_TRY(s4g_reserve(ctx, ctx->dScratchB, (size_t)len * sizeof(int32_t)));
+    const int len = (int)std::min<int64_t>({total - base, window + ctx->nP, kMaxItems});
+    S4G_TRY(s4g_reserve(ctx, ctx->dScratchB, 2 * (size_t)len * sizeof(unsigned long long)));
     if (d_sq_dist != nullptr) S4G_TRY(s4g_reserve(ctx, ctx->dScratchC, (size_t)len * sizeof(float)));
-    int32_t* keys = d_indices + base;
+    unsigned long long* keys = ctx->dScratchB.as<unsigned long long>();
     float* vals = d_sq_dist != nullptr ? d_sq_dist + base : nullptr;
-    if (chunked) {
-      S4G_CUDA(cudaMemcpyAsync(ctx->dScratchB.p, keys, (size_t)len * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
-      if (vals != nullptr)
-        S4G_CUDA(cudaMemcpyAsync(ctx->dScratchC.p, vals, (size_t)len * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    }
-    k_range_chunk<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_offsets, n, base, window, seg_begin, seg_end);
+    const unsigned blocks = (unsigned)((len + 255) / 256);
+    k_range_keys<<<blocks, 256, 0, st>>>(d_offsets, n, base, len, d_indices, jbits, keys);
     ctx->launches++;
     S4G_CUDA(cudaGetLastError());
-    cub::DoubleBuffer<int32_t> dk(keys, ctx->dScratchB.as<int32_t>());
+    cub::DoubleBuffer<unsigned long long> dk(keys, keys + len);
     cub::DoubleBuffer<float> dv(vals, ctx->dScratchC.as<float>());
     size_t bytes = 0;
     if (vals != nullptr) {
-      S4G_CUDA(cub::DeviceSegmentedSort::SortPairs(nullptr, bytes, dk, dv, len, n, seg_begin, seg_end, st));
+      S4G_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, bytes, dk, dv, len, 0, end_bit, st));
       S4G_TRY(s4g_reserve(ctx, ctx->dCub, bytes));
-      S4G_CUDA(cub::DeviceSegmentedSort::SortPairs(ctx->dCub.p, bytes, dk, dv, len, n, seg_begin, seg_end, st));
+      S4G_CUDA(cub::DeviceRadixSort::SortPairs(ctx->dCub.p, bytes, dk, dv, len, 0, end_bit, st));
     } else {
-      S4G_CUDA(cub::DeviceSegmentedSort::SortKeys(nullptr, bytes, dk, len, n, seg_begin, seg_end, st));
+      S4G_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, bytes, dk, len, 0, end_bit, st));
       S4G_TRY(s4g_reserve(ctx, ctx->dCub, bytes));
-      S4G_CUDA(cub::DeviceSegmentedSort::SortKeys(ctx->dCub.p, bytes, dk, len, n, seg_begin, seg_end, st));
+      S4G_CUDA(cub::DeviceRadixSort::SortKeys(ctx->dCub.p, bytes, dk, len, 0, end_bit, st));
     }
-    if (dk.Current() != keys)
-      S4G_CUDA(cudaMemcpyAsync(keys, dk.Current(), (size_t)len * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+    k_range_unkey<<<blocks, 256, 0, st>>>(dk.Current(), len, jmask, d_indices + base);
+    ctx->launches++;
+    S4G_CUDA(cudaGetLastError());
     if (vals != nullptr && dv.Current() != vals)
       S4G_CUDA(cudaMemcpyAsync(vals, dv.Current(), (size_t)len * sizeof(float), cudaMemcpyDeviceToDevice, st));
   }

@@ -129,14 +129,26 @@ def test_ragged_query_counts(make_ctx, n):
         assert len(got[0]) == n + 1 and got[0][0] == 0
 
 
+def lists_cut_by_a_sort(offsets, window, nP):
+    """the lists that the sort of some window leaves partly sorted (range_fill in csrc/query.cu: the sort of the window
+    starting at base covers the window + |P| entries from base), to be sorted whole by a later window's sort"""
+    total, cut = int(offsets[-1]), 0
+    for base in range(0, total, window):
+        end = min(total, base + window + nP)
+        cut += int(np.count_nonzero((offsets[:-1] < end) & (offsets[1:] > end)))
+    return cut
+
+
 def test_multi_chunk_sort_equals_single(make_ctx):
     """the per-list sort in windows (the path of results over 2^31 entries, here forced by a small window): the same
-    lists as one window"""
+    lists as one window, with lists cut off at the end of a window's sort"""
     sc = common.scenario(20000, 0.4, 0.01, seed=6)
     X = queries(sc["P"], 0.01, np.random.RandomState(5), 2000, 100, 100)
     r = 0.08 ** 2
     want = orange.bruteforce(sc["P"], X, r)
     assert want[0][-1] > 80000
+    for window in (997, 40000):
+        assert lists_cut_by_a_sort(want[0], window, len(sc["P"])) > 0, window
     for window in (None, 997, 40000):
         ctx = make_ctx(sort_window=window)
         ctx.set_cloud_p(sc["P"], 0.01)
